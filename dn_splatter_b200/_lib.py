@@ -84,6 +84,19 @@ KERNELS_PER_CALL = {
     "dnr_knn_build": (2, 1), "dnr_knn_query": (1, 0), "dnr_density": (1, 0), "dnr_ray_densities": (1, 0),
 }
 LAUNCHES = {"handwritten": 0, "cub": 0}
+DEBUG_CAPTURE = os.environ.get("DNR_DEBUG_CAPTURE") == "1"
+
+
+def capture_ok(where: str) -> None:
+    """With DEBUG_CAPTURE set: raises, naming `where`, once an ongoing stream capture is no longer valid."""
+    if not DEBUG_CAPTURE:
+        return
+    import torch
+
+    try:  # raises cudaErrorStreamCaptureInvalidated once the capture is broken
+        torch.cuda.is_current_stream_capturing()
+    except Exception as exc:  # noqa: BLE001
+        raise DnrError(f"stream capture invalidated by {where}: {exc}") from exc
 
 
 class _Counting:
@@ -98,19 +111,12 @@ class _Counting:
         if k is None:
             return fn
 
-        debug = os.environ.get("DNR_DEBUG_CAPTURE") == "1"
-
         def call(*args):
             LAUNCHES["handwritten"] += k[0]
             LAUNCHES["cub"] += k[1]
             rc = fn(*args)
-            if debug:  # name the C-ABI call that invalidates an ongoing stream capture
-                import torch
-
-                try:  # raises cudaErrorStreamCaptureInvalidated once the capture is broken
-                    torch.cuda.is_current_stream_capturing()
-                except Exception as exc:  # noqa: BLE001
-                    raise DnrError(f"stream capture invalidated by {name} (rc {rc}): {exc}") from exc
+            if DEBUG_CAPTURE:  # name the C-ABI call that invalidates an ongoing stream capture
+                capture_ok(f"{name} (rc {rc})")
             return rc
 
         self.__dict__[name] = call

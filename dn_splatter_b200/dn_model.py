@@ -421,7 +421,7 @@ class DNSplatterModel(_ModelBase):
         fixed_capacity = 0
         gc = self.__dict__.get("_graph_cam")
         if gc is not None:  # CUDA-graph mode: camera in static device buffers (refreshed before each replay), fixed capacity
-            K, c2w_fixed, viewmat, fixed_capacity = gc["K"], gc["c2w"], gc["viewmat"], gc["capacity"]
+            K, c2w_fixed, viewmat, fixed_capacity = gc.K, gc.c2w, gc.viewmat, gc.capacity
         self.last_size = (H, W)
         camera.rescale_output_resolution(scale_fac)
         sh_degree_to_use = min(self.step // cfg.sh_degree_interval, cfg.sh_degree)

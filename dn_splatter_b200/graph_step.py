@@ -1,14 +1,14 @@
 """CUDA-graph capture of one whole training view: bucket.zero_ -> get_outputs -> get_loss_dict -> backward
 (-> the caller's all-reduce / optimiser outside the graph).  ~46 kernel launches, ~60 allocations and ~1.3 ms of
 Python per view collapse into one cudaGraphLaunch, which makes the step immune to host jitter and removes the
-inter-kernel launch gaps.
+inter-kernel launch gaps.  render_service.py captures its forward with the same StaticCamera and capture_slots.
 
 What makes the step capturable (see rasterize.py / dn_model.py):
   * `fixed_capacity`: intersection buffers sized once (1.15 x the largest count seen), no count read-back inside the
-    graph; after every replay the view's count is copied to pinned memory asynchronously and checked at the NEXT call
-    (and by `check_capacity()`): a replay that needed more slots raises DnrCapacityError — call `recapture()` and redo;
-  * the camera lives in static device tensors (viewmat, K, c2w) that `load_camera` refreshes with one small
-    pinned H2D copy before each replay (resolution must not change between replays);
+    graph; every replay's count goes to a rasterize.CountWatch, checked at the NEXT call (and by `check_capacity()`):
+    a replay that needed more slots raises DnrCapacityError — call `recapture()` and redo;
+  * the camera lives in a StaticCamera that `load_camera` refreshes with one small pinned H2D copy before each
+    replay (resolution must not change between replays);
   * the supervision maps live in static device buffers that the caller fills (H2D or D2D) before each replay;
   * gradients go to the flat bucket (static addresses); the loss is a static 0-dim tensor.
 Run the training loop on a non-default stream (`torch.cuda.set_stream(torch.cuda.Stream())`): the legacy default
@@ -17,12 +17,58 @@ first used on.
 """
 from __future__ import annotations
 
-from typing import Dict, List, Optional
+from typing import Dict, List, Optional, Tuple
 
 import torch
 from torch import Tensor
 
-from .rasterize import DnrCapacityError, get_viewmat, round_capacity, suggested_capacity
+from . import _lib as L
+from .rasterize import GROWTH, CountWatch, get_viewmat, grow, suggested_capacity
+
+
+class StaticCamera:
+    """What get_outputs renders with while installed as the model's `_graph_cam`: the static device camera block
+    [viewmat 16 | K 9 | c2w 12], read through `viewmat` / `K` / `c2w`, and the graph's fixed intersection `capacity`."""
+
+    def __init__(self, size: Tuple[int, int], device, capacity: int):
+        self.size, self.capacity = size, int(capacity)
+        self.data = torch.zeros(37, device=device)
+        self.viewmat, self.K, self.c2w = self.data[:16].view(4, 4), self.data[16:25].view(3, 3), self.data[25:].view(3, 4)
+
+    def load(self, camera) -> None:
+        """Refreshes the block from a camera: ONE 148-byte async H2D copy from a per-camera pinned tensor
+        (stream-ordered after the previous replay, so the host may run ahead)."""
+        assert (int(camera.width.flatten()[0]), int(camera.height.flatten()[0])) == self.size, "resolution is baked in"
+        pinned = camera.__dict__.get("_dnr_graph_cam")
+        if pinned is None:
+            c2w = camera.camera_to_worlds.reshape(-1, 3, 4)[0].detach().float().cpu()
+            pinned = torch.cat([get_viewmat(c2w).reshape(-1), camera.get_intrinsics_matrices()[0].float().cpu().reshape(-1),
+                                c2w.reshape(-1)]).contiguous().pin_memory()
+            camera.__dict__["_dnr_graph_cam"] = pinned
+        self.data.copy_(pinned, non_blocking=True)
+
+
+def capture_slots(fn, n_slots: int, warmup: int, device) -> Tuple[List[torch.cuda.CUDAGraph], list]:
+    """Runs `fn(0)` `warmup` times on a side stream (allocator pools, cub temp sizes), then captures `fn(slot)` once per
+    slot into graphs that share one memory pool; returns the graphs and what each captured call returned."""
+    side = torch.cuda.Stream(device=device)
+    side.wait_stream(torch.cuda.current_stream())
+    with torch.cuda.stream(side):
+        for _ in range(warmup):
+            fn(0)
+    torch.cuda.current_stream().wait_stream(side)
+    torch.cuda.synchronize(device)
+    # thread-local capture mode: other threads of the process (NCCL's watchdog, the symmetric-memory runtime of a
+    # multi-rank job) keep making CUDA API calls while we capture; in the default "global" mode any of them invalidates
+    # the capture (cudaErrorStreamCaptureInvalidated, seen intermittently at 2 ranks)
+    graphs, results, pool = [], [], None
+    for slot in range(n_slots):
+        g = torch.cuda.CUDAGraph()
+        with torch.cuda.graph(g, pool=pool, capture_error_mode="thread_local"):
+            results.append(fn(slot))
+        pool = g.pool()
+        graphs.append(g)
+    return graphs, results
 
 
 class GraphedTrainStep:
@@ -33,37 +79,34 @@ class GraphedTrainStep:
             raise ValueError("background_color='random' draws a new host-side colour every step; a captured graph would "
                              "freeze the first one.  Use 'black' / 'white' (or run eagerly).")
         self.model, self.bucket = model, bucket
-        dev = model.device
-        self.device = dev
+        dev = self.device = model.device
         W, H = int(example_camera.width.flatten()[0]), int(example_camera.height.flatten()[0])
-        self.size = (W, H)
         if capacity is None:
-            capacity = suggested_capacity(model.num_points, W, H, model.config.predict_normals,
-                                          model.config.exact_isect_lists, dev.index,
-                                          0 if model.config.exact_isect_lists else model.config.list_shift)
+            cfg = model.config
+            capacity = suggested_capacity(model.num_points, W, H, cfg.predict_normals, cfg.exact_isect_lists, dev.index,
+                                          cfg.list_shift)
         if capacity <= 0:
             raise ValueError("no intersection statistics yet: run a few sync_free views first or pass capacity=")
-        self.capacity = int(capacity)
-        # one static device block [viewmat 16 | K 9 | c2w 12]; the kernels read the camera through these views
-        self._cam_dev = torch.zeros(37, device=dev)
-        self.cam = {"viewmat": self._cam_dev[:16].view(4, 4), "K": self._cam_dev[16:25].view(3, 3),
-                    "c2w": self._cam_dev[25:37].view(3, 4), "capacity": self.capacity}
+        self.cam = StaticCamera((W, H), dev, capacity)
         self.batches: List[Dict[str, Tensor]] = [
             {k: torch.empty_like(v, device=dev) for k, v in example_batch.items()} for _ in range(n_slots)]
         self.losses = [torch.zeros((), device=dev) for _ in range(n_slots)]
-        self.graphs: List[torch.cuda.CUDAGraph] = []
         self._camera = example_camera
         self._n_slots, self._warmup = n_slots, warmup
-        self._count_dev: List[Optional[Tensor]] = [None] * n_slots   # the graphs' own n_isects_dev tensors
-        self._count_host = torch.zeros(64, dtype=torch.int64).pin_memory()
-        self._count_pending: List = []
-        self._count_slot = 0
-        self.max_count = 0
+        self._watch = CountWatch("Call recapture() and run the view again.")
         for b in self.batches:
             for k, v in example_batch.items():
                 b[k].copy_(v)
         self.load_camera(example_camera)
         self._capture()
+
+    @property
+    def capacity(self) -> int:
+        return self.cam.capacity
+
+    @property
+    def max_count(self) -> int:
+        return self._watch.max_seen
 
     @staticmethod
     def _gates(m):
@@ -73,10 +116,8 @@ class GraphedTrainStep:
                 bool(c.use_binary_opacities and m.step > c.warmup_length), m._get_downscale_factor())
 
     def _capture(self) -> None:
-        model, dev = self.model, self.device
+        model = self.model
         self._captured_gates = self._gates(model)
-        warmup, n_slots = self._warmup, self._n_slots
-        self.cam["capacity"] = self.capacity
         self.graphs = []
         # Autograd graphs of earlier eager steps keep the parameters' AccumulateGrad nodes alive, and those remember the
         # stream they were created on (usually the legacy default stream, which may not take part in a capture):
@@ -87,66 +128,29 @@ class GraphedTrainStep:
             if name in model.__dict__:
                 model.__dict__[name] = None
         gc.collect()
-        # warm-up on a side stream (allocator pools, cub temp sizes), then one graph per batch slot
-        side = torch.cuda.Stream(device=dev)
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(warmup):
-                self._eager(0)
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize(dev)
-        # capture_error_mode="thread_local": other threads of the process (NCCL's watchdog, the symmetric-memory runtime of a
-        # multi-rank job) keep making CUDA API calls while we capture; in the default "global" mode any of them invalidates
-        # the capture (cudaErrorStreamCaptureInvalidated, seen intermittently at 2 ranks)
-        pool = None
-        for slot in range(n_slots):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, pool=pool, capture_error_mode="thread_local"):
-                self._eager(slot)
-            pool = g.pool()
-            self.graphs.append(g)
+        self.graphs, self._count_dev = capture_slots(self._eager, self._n_slots, self._warmup, self.device)
 
-    @staticmethod
-    def _capture_ok(where: str) -> None:
-        """DNR_DEBUG_CAPTURE=1: name the first stage after which an ongoing stream capture is no longer valid."""
-        import os
-
-        if os.environ.get("DNR_DEBUG_CAPTURE") != "1":
-            return
-        try:  # raises cudaErrorStreamCaptureInvalidated once the capture is broken
-            torch.cuda.is_current_stream_capturing()
-        except Exception as exc:  # noqa: BLE001
-            raise RuntimeError(f"stream capture invalidated during: {where}: {exc}") from exc
-
-    def _eager(self, slot: int) -> None:
+    def _eager(self, slot: int) -> Tensor:
         m = self.model
         m.__dict__["_graph_cam"] = self.cam
         try:
             self.bucket.flat.zero_()
-            self._capture_ok("bucket zero")
+            L.capture_ok("bucket zero")
             out = m.get_outputs(self._camera)
-            self._capture_ok("get_outputs")
+            L.capture_ok("get_outputs")
             ld = m.get_loss_dict(out, dict(self.batches[slot]))
-            self._capture_ok("get_loss_dict")
+            L.capture_ok("get_loss_dict")
             loss = ld["main_loss"] + ld["scale_reg"]
             loss.backward()
-            self._capture_ok("backward")
+            L.capture_ok("backward")
             self.losses[slot].copy_(loss.detach())
-            self._count_dev[slot] = m.raster_out.info["n_isects_dev"]
+            return m.raster_out.info["n_isects_dev"]  # the graph's own count tensor
         finally:
             m.__dict__["_graph_cam"] = None
 
     def load_camera(self, camera) -> None:
-        """Refreshes the static camera block from a camera: ONE 148-byte async H2D copy from a per-camera pinned tensor
-        (stream-ordered after the previous replay, so the host may run ahead)."""
-        assert (int(camera.width.flatten()[0]), int(camera.height.flatten()[0])) == self.size, "resolution is baked in"
-        pinned = camera.__dict__.get("_dnr_graph_cam")
-        if pinned is None:
-            c2w = camera.camera_to_worlds.reshape(-1, 3, 4)[0].detach().float().cpu()
-            pinned = torch.cat([get_viewmat(c2w).reshape(-1), camera.get_intrinsics_matrices()[0].float().cpu().reshape(-1),
-                                c2w.reshape(-1)]).contiguous().pin_memory()
-            camera.__dict__["_dnr_graph_cam"] = pinned
-        self._cam_dev.copy_(pinned, non_blocking=True)
+        """Refreshes the static camera block from a camera (StaticCamera.load)."""
+        self.cam.load(camera)
 
     def __call__(self, camera, slot: int = 0) -> Tensor:
         """Replays the captured step for `camera` on the supervision maps currently in `self.batches[slot]`;
@@ -157,37 +161,20 @@ class GraphedTrainStep:
         self.check_capacity()
         self.load_camera(camera)
         self.graphs[slot].replay()
-        host = self._count_host[self._count_slot:self._count_slot + 1]
-        self._count_slot = (self._count_slot + 1) % self._count_host.numel()
-        host.copy_(self._count_dev[slot], non_blocking=True)
-        ev = torch.cuda.Event()
-        ev.record()
-        self._count_pending.append((host, ev))
-        if len(self._count_pending) >= self._count_host.numel() - 1:
-            self.check_capacity(wait=True)
+        self._watch.observe(self._count_dev[slot], self.capacity)
         return self.losses[slot]
 
     def check_capacity(self, wait: bool = False) -> None:
         """Raises DnrCapacityError if a finished replay needed more intersection slots than the graph was captured
         with (its gradients are truncated: discard them, `recapture()`, replay the view again)."""
-        keep, worst = [], 0
-        for host, ev in self._count_pending:
-            if wait:
-                ev.synchronize()
-            if ev.query():
-                worst = max(worst, int(host.item()))
-            else:
-                keep.append((host, ev))
-        self._count_pending = keep
-        self.max_count = max(self.max_count, worst)
-        if worst > self.capacity:
-            raise DnrCapacityError(f"a replayed view needed {worst} intersection slots, the graph holds {self.capacity}: "
-                                   "its outputs and gradients are truncated; call recapture() and run the view again")
+        self._watch.poll(wait)
+        self._watch.raise_unreported()
 
     def recapture(self, capacity: Optional[int] = None) -> None:
-        """Re-captures the step with room for the largest count seen so far (x 1.15) or the given capacity."""
-        need = int(capacity) if capacity else round_capacity(int(self.max_count * 1.15) + 4096)
-        self.capacity = max(self.capacity, need)
-        self._count_pending = []
+        """Re-captures the step with room for the largest count seen so far (grow(.., GROWTH)) or the given capacity."""
+        self._watch.poll(wait=True)
+        self._watch.unreported = None  # an overflow of the old graphs: the caller runs that view again
+        need = int(capacity) if capacity else grow(self.max_count, GROWTH)
+        self.cam.capacity = max(self.cam.capacity, need)
         torch.cuda.synchronize(self.device)
         self._capture()

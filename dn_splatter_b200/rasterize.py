@@ -29,39 +29,31 @@ class DnrCapacityError(L.DnrError):
     truncated and must not be used.  The capacity has already been raised; render the view again."""
 
 
-class _CapacityTracker:
-    """Sync-free sizing of the intersection buffers: the count of every view is copied to pinned host memory
-    asynchronously; capacity for the next view = 1.15 x the largest count seen so far (rounded up).  A view whose
-    count exceeded its capacity was rendered without its farthest intersections: that is never silent — the view's
-    own backward (or the next forward, for no-grad renders) raises DnrCapacityError before any gradient is produced."""
+class CountWatch:
+    """Host-side overflow check of fixed-capacity intersection buffers, whose binning kernels silently drop the entries
+    past the capacity.  Each view's count is copied to a pinned ring asynchronously (`observe`); `check` raises
+    DnrCapacityError for a truncated view, and a truncated view nobody checked is kept for `raise_unreported`."""
 
     SLOTS = 256
 
-    def __init__(self):
+    def __init__(self, remedy: str = ""):
+        self.remedy = remedy  # what the error message tells the user to do
         self.max_seen, self.overflows, self.pending, self.seeds = 0, 0, [], 0
-        self.host, self.slot = None, 0
-        self.unreported = None  # (needed, capacity) of a truncated no-grad view nobody has been told about yet
+        self.host, self.slot = torch.zeros(self.SLOTS, dtype=torch.int64).pin_memory(), 0
+        self.unreported = None  # (needed, capacity) of a truncated view whose ticket nobody has checked
 
-    def seed(self, count: int):
+    def seed(self, count: int) -> None:
+        """Records a count that was read back synchronously."""
         self.max_seen = max(self.max_seen, count)
         self.seeds += 1
 
-    def ready(self) -> bool:
-        self.drain()
-        return self.seeds >= 2
-
-    def capacity(self) -> int:
-        return round_capacity(int(self.max_seen * 1.15) + 4096)
-
-    def observe(self, n_isects_dev: Tensor, cap: int):
-        """Queues the async read-back of this view's count; returns the ticket its backward checks."""
-        if self.host is None:
-            self.host = torch.zeros(self.SLOTS, dtype=torch.int64).pin_memory()
+    def observe(self, count_dev: Tensor, cap: int) -> dict:
+        """Queues the async read-back of `count_dev` (int64[1]) on the current stream; returns its ticket."""
         if len(self.pending) >= self.SLOTS - 1:
-            self.drain(wait=True)
+            self.poll(wait=True)
         host = self.host[self.slot:self.slot + 1]
         self.slot = (self.slot + 1) % self.SLOTS
-        host.copy_(n_isects_dev, non_blocking=True)
+        host.copy_(count_dev, non_blocking=True)
         ev = torch.cuda.Event()
         ev.record()
         ticket = {"host": host, "event": ev, "cap": cap, "count": None, "checked": False}
@@ -77,7 +69,8 @@ class _CapacityTracker:
                 if not t["checked"]:
                     self.unreported = (t["count"], t["cap"])
 
-    def drain(self, wait: bool = False):
+    def poll(self, wait: bool = False) -> None:
+        """Resolves the tickets whose copies have landed (all pending tickets with wait=True)."""
         keep = []
         for t in self.pending:
             if wait:
@@ -89,28 +82,24 @@ class _CapacityTracker:
         self.pending = keep
 
     def check(self, ticket) -> None:
-        """Called by the view's own backward: waits for ITS count (recorded right after bin_scan, long passed by the
-        time the loss has been enqueued) and raises if the view was truncated."""
+        """Waits for this ticket's count and raises DnrCapacityError if its view was truncated."""
         ticket["checked"] = True
         ticket["event"].synchronize()
         self._resolve(ticket)
-        if self.unreported is not None and self.unreported == (ticket["count"], ticket["cap"]):
+        if self.unreported == (ticket["count"], ticket["cap"]):
             self.unreported = None
         if ticket["count"] > ticket["cap"]:
-            raise DnrCapacityError(
-                f"this view needs {ticket['count']} intersection slots but was rendered with {ticket['cap']}: outputs and "
-                "gradients are truncated.  The capacity has been raised — run the view again (or use sync_free=False).")
+            raise DnrCapacityError(f"this view needs {ticket['count']} intersection slots but was rendered with "
+                                   f"{ticket['cap']}: its outputs and gradients are truncated.  {self.remedy}")
 
     def raise_unreported(self) -> None:
         if self.unreported is not None:
-            need, cap = self.unreported
-            self.unreported = None
-            raise DnrCapacityError(
-                f"an earlier no-grad view needed {need} intersection slots but was rendered with {cap}: that render was "
-                "truncated.  The capacity has been raised — render it again.")
+            (need, cap), self.unreported = self.unreported, None
+            raise DnrCapacityError(f"an earlier view needed {need} intersection slots but was rendered with {cap}: its "
+                                   f"outputs and gradients are truncated.  {self.remedy}")
 
 
-_CAPACITY: dict = {}
+GROWTH = 1.15  # headroom over the largest count seen: sync-free sizing and training-graph re-capture
 
 
 def round_capacity(need: int) -> int:
@@ -121,15 +110,26 @@ def round_capacity(need: int) -> int:
     return (need + step - 1) // step * step
 
 
+def grow(count: int, factor: float) -> int:
+    """Intersection capacity with room for `count` times `factor`, plus a fixed margin, rounded up."""
+    return round_capacity(int(count * factor) + 4096)
+
+
+# Sync-free sizing: one CountWatch per (device, n, W, H, normals, exact lists, list tile).  After two synchronous views a
+# view gets grow(max count seen, GROWTH) slots; if truncated, its backward (no-grad: the next forward) raises.
+_CAPACITY: dict = {}
+
+
 def suggested_capacity(n_gauss: int, width: int, height: int, render_normals: bool = True, exact_lists: bool = False,
                        device_index: Optional[int] = None, list_shift: Optional[int] = None) -> int:
-    """Capacity (1.15 x the largest intersection count seen in sync-free mode, rounded up) for graph capture."""
+    """Capacity for graph capture: grow(largest count seen in sync-free mode, GROWTH), 0 without statistics.
+    `list_shift` is ignored with exact_lists, which always bins per 16-pixel tile."""
     best = 0
     for (di, n, w, h, rn, ex, lt), t in _CAPACITY.items():
         if (n, w, h, rn, ex) == (n_gauss, width, height, render_normals, exact_lists) and (device_index in (None, di)) \
-                and (list_shift is None or lt == TILE << list_shift):
-            t.drain(wait=True)
-            best = max(best, t.capacity())
+                and (list_shift is None or exact_lists or lt == TILE << list_shift):
+            t.poll(wait=True)
+            best = max(best, grow(t.max_seen, GROWTH))
     return best
 
 
@@ -137,7 +137,7 @@ def capacity_report() -> dict:
     """{key: (max intersections seen, truncated views)} for the sync-free mode; waits for pending counts."""
     out = {}
     for k, t in _CAPACITY.items():
-        t.drain(wait=True)
+        t.poll(wait=True)
         out[k] = (t.max_seen, t.overflows)
     return out
 
@@ -320,29 +320,31 @@ class _DnRasterize(torch.autograd.Function):
         ws_scan = torch.empty(lib.dnr_bin_scan_workspace_bytes(n), dtype=torch.uint8, device=dev)
         _set(a, ws_scan=ws_scan)
         cap_key = (dev.index, n, W, H, s.render_normals, s.exact_lists, list_tile)
-        tracker = _CAPACITY.get(cap_key) if s.sync_free else None
+        watch = _CAPACITY.get(cap_key) if s.sync_free else None
         if s.fixed_capacity > 0:
-            # graph-capturable: no read-back, no events, no host state; the owner of the graph (graph_step.py) watches
-            # info["n_isects_dev"] and raises DnrCapacityError when a replay needed more slots
+            # graph-capturable: no read-back, no events, no host state; the owner of the graph (graph_step.py,
+            # render_service.py) gives the replay's info["n_isects_dev"] to a CountWatch
             L.check(_timed("bin_scan", lib.dnr_bin_scan, C.byref(a), st, None), "dnr_bin_scan")
             n_isects = int(s.fixed_capacity)
-        elif tracker is not None and tracker.ready():
+        elif watch is not None and watch.seeds >= 2:
             # sync-free: nothing is read back on this stream; capacity comes from the counts of earlier views
-            tracker.raise_unreported()
+            watch.poll()
+            watch.raise_unreported()
             L.check(_timed("bin_scan", lib.dnr_bin_scan, C.byref(a), st, None), "dnr_bin_scan")
-            n_isects = tracker.capacity()
-            ctx.capacity_ticket = (tracker, tracker.observe(n_isects_dev, n_isects))
+            n_isects = grow(watch.max_seen, GROWTH)
+            ctx.capacity_ticket = (watch, watch.observe(n_isects_dev, n_isects))
         else:
             total = C.c_int64(0)
             L.check(_timed("bin_scan", lib.dnr_bin_scan, C.byref(a), st, C.byref(total)), "dnr_bin_scan")
             n_isects = int(total.value)
             if s.sync_free:
                 if cap_key not in _CAPACITY:
-                    # the Gaussian count changed (densification): drop the trackers of the old counts for this
+                    # the Gaussian count changed (densification): drop the watches of the old counts for this
                     # device / resolution instead of keeping one pinned buffer per count ever seen
                     for stale in [k for k in _CAPACITY if k[0] == cap_key[0] and k[2:] == cap_key[2:] and k[1] != n]:
                         del _CAPACITY[stale]
-                    _CAPACITY[cap_key] = _CapacityTracker()
+                    _CAPACITY[cap_key] = CountWatch("The capacity has been raised — render the view again "
+                                                    "(or use sync_free=False).")
                 _CAPACITY[cap_key].seed(n_isects)
         a.n_isects = n_isects
         ws_sort = torch.empty(lib.dnr_bin_sort_workspace_bytes(n, n_isects, n_tiles), dtype=torch.uint8, device=dev)
@@ -399,8 +401,8 @@ class _DnRasterize(torch.autograd.Function):
         lib = L.load()
         s: RasterSettings = ctx.settings
         if ctx.capacity_ticket is not None:  # sync-free sizing: never produce gradients from a truncated render
-            tracker, ticket = ctx.capacity_ticket
-            tracker.check(ticket)
+            watch, ticket = ctx.capacity_ticket
+            watch.check(ticket)
         means, quats, scales, opac, sh_dc, sh_rest, viewmat, K, c2w = ctx.saved_tensors
         S = ctx.state
         n, dev = ctx.n, means.device

@@ -7,8 +7,9 @@ surface normal, ~20 launches and ~1 ms of Python) is captured ONCE per resolutio
 that write into their own static output maps; a view is then one 148-byte camera upload + one graph launch.  With
 `to_host=True` the selected maps of slot s are copied to pinned host buffers on a side stream while slot s+1 renders, and
 a view is handed out when its copy has landed.  The intersection buffers have a fixed capacity inside a graph: every
-replay's count is read back with the maps, and a view that needed more is re-rendered after re-capturing with a larger
-capacity — the consumer never sees a truncated render.
+replay's count goes to a rasterize.CountWatch on the copy stream, and a view that needed more is rendered again after
+re-capturing with a larger capacity — the consumer never sees a truncated render.  The static camera block and the
+capture recipe are graph_step.py's.
 
 `graph=False` is the plain loop (also what non-CUDA models, i.e. the CPU-proxy tests, use).
 """
@@ -19,30 +20,23 @@ from typing import Dict, Iterable, Iterator, List, Optional, Sequence, Tuple
 import torch
 from torch import Tensor
 
+from .graph_step import StaticCamera, capture_slots
+from .rasterize import CountWatch, DnrCapacityError, grow, suggested_capacity
+
 DEFAULT_KEYS = ("rgb", "depth", "normal", "surface_normal", "accumulation")
+RENDER_GROWTH = 1.3  # headroom over the count of an overflowing view (or, without statistics, of the first view)
 
 
 class _ForwardGraphs:
     """`n_slots` captured copies of model.get_outputs for one resolution."""
 
     def __init__(self, model, camera, keys: Sequence[str], n_slots: int, capacity: int):
-        from .graph_step import GraphedTrainStep  # camera block upload is shared
-
         self.model, self.keys, self.n_slots = model, tuple(keys), n_slots
-        self.device = model.device
-        self.size = (int(camera.width.flatten()[0]), int(camera.height.flatten()[0]))
-        self.capacity = int(capacity)
-        self._cam_dev = torch.zeros(37, device=self.device)
-        self.cam = {"viewmat": self._cam_dev[:16].view(4, 4), "K": self._cam_dev[16:25].view(3, 3),
-                    "c2w": self._cam_dev[25:37].view(3, 4), "capacity": self.capacity}
+        self.cam = StaticCamera((int(camera.width.flatten()[0]), int(camera.height.flatten()[0])), model.device, capacity)
         self._camera = camera
-        self._load_camera = GraphedTrainStep.load_camera.__get__(self)  # same pinned 148-byte upload
-        self.graphs: List[torch.cuda.CUDAGraph] = []
-        self.maps: List[Dict[str, Tensor]] = []
-        self.counts: List[Tensor] = []
         self._capture()
 
-    def _eager(self) -> Tuple[Dict[str, Tensor], Tensor]:
+    def _eager(self, slot: int) -> Tuple[Dict[str, Tensor], Tensor]:
         m = self.model
         m.__dict__["_graph_cam"] = self.cam
         try:
@@ -53,28 +47,10 @@ class _ForwardGraphs:
 
     @torch.no_grad()
     def _capture(self) -> None:
-        self.cam["capacity"] = self.capacity
-        self._load_camera(self._camera)
-        side = torch.cuda.Stream(device=self.device)
-        side.wait_stream(torch.cuda.current_stream())
-        with torch.cuda.stream(side):
-            for _ in range(2):
-                self._eager()
-        torch.cuda.current_stream().wait_stream(side)
-        torch.cuda.synchronize(self.device)
-        self.graphs, self.maps, self.counts, pool = [], [], [], None
-        for _ in range(self.n_slots):
-            g = torch.cuda.CUDAGraph()
-            with torch.cuda.graph(g, pool=pool, capture_error_mode="thread_local"):
-                maps, count = self._eager()
-            pool = g.pool()
-            self.graphs.append(g)
-            self.maps.append(maps)
-            self.counts.append(count)
-
-    def replay(self, camera, slot: int) -> None:
-        self._load_camera(camera)
-        self.graphs[slot].replay()
+        self.cam.load(self._camera)
+        self.graphs = self.maps = self.counts = ()  # release the old graphs and their maps before capturing new ones
+        self.graphs, outs = capture_slots(self._eager, self.n_slots, 2, self.model.device)
+        self.maps, self.counts = zip(*outs)  # per slot: the static output maps and the intersection count
 
 
 class ViewRenderer:
@@ -123,21 +99,17 @@ class ViewRenderer:
 
     # ------------------------------------------------------------------ captured forward
     def _graphs_for(self, cam) -> _ForwardGraphs:
-        from .rasterize import suggested_capacity
-
         m = self.model
         key = (int(cam.width.flatten()[0]), int(cam.height.flatten()[0]))
         fg = self._graphs.get(key)
         if fg is None or fg.model.num_points != m.num_points:
             cfg = m.config
-            with torch.no_grad():  # two synchronous views seed the capacity statistics for this size if there are none
+            with torch.no_grad():  # without sync-free statistics for this size, one synchronous view sizes the capacity
                 cap = suggested_capacity(m.num_points, key[0], key[1], cfg.predict_normals, cfg.exact_isect_lists, m.device.index,
-                                         0 if cfg.exact_isect_lists else cfg.list_shift)
+                                         cfg.list_shift)
                 if cap <= 0:
-                    from .rasterize import round_capacity
-
                     m.get_outputs(cam)
-                    cap = round_capacity(int(int(m.raster_out.info["n_isects_dev"]) * 1.3) + 4096)
+                    cap = grow(int(m.raster_out.info["n_isects_dev"]), RENDER_GROWTH)
             fg = self._graphs[key] = _ForwardGraphs(m, cam, self.keys, self.n_slots, cap)
         return fg
 
@@ -150,11 +122,12 @@ class ViewRenderer:
         copy_stream = torch.cuda.Stream(device=dev)
         compute = torch.cuda.current_stream()
         n_slots = self.n_slots
-        host = [None] * n_slots            # pinned {key: tensor, "_count": int64[1]} per slot
+        watch = CountWatch()
+        host = [None] * n_slots            # pinned {key: tensor} per slot (to_host)
         rendered = [torch.cuda.Event() for _ in range(n_slots)]
         copied = [torch.cuda.Event() for _ in range(n_slots)]
         busy = [False] * n_slots
-        inflight: List[Tuple[int, int, _ForwardGraphs]] = []  # (view index, slot, graphs) in submission order
+        inflight: List[Tuple[int, int, _ForwardGraphs, dict]] = []  # (view index, slot, graphs, count ticket) in order
 
         def submit(idx):
             cam = cams[idx]
@@ -162,52 +135,39 @@ class ViewRenderer:
             slot = idx % n_slots
             if busy[slot]:
                 compute.wait_event(copied[slot])  # the copy that still reads this slot's static maps
-            fg.replay(cam, slot)
+            fg.cam.load(cam)
+            fg.graphs[slot].replay()
             rendered[slot].record(compute)
-            if host[slot] is None or any(host[slot][k].shape != v.shape for k, v in fg.maps[slot].items()):
+            if self.to_host and (host[slot] is None or any(host[slot][k].shape != v.shape for k, v in fg.maps[slot].items())):
                 host[slot] = {k: torch.empty(v.shape, dtype=v.dtype).pin_memory() for k, v in fg.maps[slot].items()}
-                host[slot]["_count"] = torch.zeros(1, dtype=torch.int64).pin_memory()
             with torch.cuda.stream(copy_stream):
                 copy_stream.wait_event(rendered[slot])
-                host[slot]["_count"].copy_(fg.counts[slot], non_blocking=True)
+                ticket = watch.observe(fg.counts[slot], fg.cam.capacity)
                 if self.to_host:
                     for k, v in fg.maps[slot].items():
                         host[slot][k].copy_(v, non_blocking=True)
                 copied[slot].record(copy_stream)
             busy[slot] = True
-            inflight.append((idx, slot, fg))
+            inflight.append((idx, slot, fg, ticket))
 
         def collect():
-            idx, slot, fg = inflight.pop(0)
+            idx, slot, fg, ticket = inflight.pop(0)
             copied[slot].synchronize()
-            need = int(host[slot]["_count"])
-            if need > fg.capacity:  # truncated: grow, re-capture, render this view again (synchronously)
-                from .rasterize import round_capacity
-
-                for _, s2, _ in inflight:  # drain what is in flight on the old graphs first
+            try:
+                watch.check(ticket)
+            except DnrCapacityError:  # truncated: grow, re-capture, and submit this view and those in flight again
+                for _, s2, _, _ in inflight:  # drain what is in flight on the old graphs first
                     copied[s2].synchronize()
-                fg.capacity = round_capacity(int(need * 1.3) + 4096)
+                fg.cam.capacity = grow(ticket["count"], RENDER_GROWTH)
                 fg._capture()
                 self.recaptures += 1
-                redo = [idx] + [i for i, _, _ in inflight]
+                redo = [idx] + [i for i, _, _, _ in inflight]
                 inflight.clear()
-                for s2 in range(n_slots):
-                    busy[s2] = False
-                out = None
-                for j in redo:  # serial re-render of the affected window keeps the order
+                busy[:] = [False] * n_slots
+                for j in redo:  # back in flight in order; collect() checks each of them again
                     submit(j)
-                    i2, s2, fg2 = inflight.pop(0)
-                    copied[s2].synchronize()
-                    maps = ({k: v.clone() for k, v in host[s2].items() if k != "_count"} if self.to_host
-                            else {k: v.clone() for k, v in fg2.maps[s2].items()})
-                    if out is None:
-                        out = [(i2, maps)]
-                    else:
-                        out.append((i2, maps))
-                return out
-            if self.to_host:
-                return [(idx, {k: v for k, v in host[slot].items() if k != "_count"})]
-            return [(idx, fg.maps[slot])]
+                return None
+            return idx, (host[slot] if self.to_host else fg.maps[slot])
 
         depth = n_slots - 1 if self.to_host else 0  # views in flight while the caller consumes one
         nxt = 0
@@ -215,7 +175,8 @@ class ViewRenderer:
             while nxt < len(cams) and len(inflight) <= depth:
                 submit(nxt)
                 nxt += 1
-            for item in collect():
+            item = collect()
+            if item is not None:
                 yield item
 
     @torch.no_grad()

@@ -190,12 +190,21 @@ def test_cuda_graph_step_matches_eager_step():
         _graph_step_body()
 
 
-def _graph_step_body():
+@needs_cuda
+def test_graphed_train_step_overflow_is_loud_and_recoverable():
+    """A training graph captured with far fewer intersection slots than the view needs: the truncated replay is reported
+    by check_capacity (DnrCapacityError), and after recapture() the replays reproduce the eager loss and gradients."""
+    with torch.cuda.stream(torch.cuda.Stream()):
+        _graph_step_body(n_gauss=12000, capacity=4096)
+
+
+def _graph_step_body(n_gauss=4000, capacity=None):
     from dn_splatter_b200.graph_step import GraphedTrainStep
     from dn_splatter_b200.losses import DepthLossType
+    from dn_splatter_b200.rasterize import DnrCapacityError
     from dn_splatter_b200.synthetic import ring_cameras
 
-    params, _ = scene_and_camera(4000, 160, 128)
+    params, _ = scene_and_camera(n_gauss, 160, 128)
     cams = [_camera(c) for c in ring_cameras(6, 160, 128)]
     for c in cams:
         c.camera_to_worlds = c.camera_to_worlds.cpu()
@@ -204,19 +213,30 @@ def _graph_step_body():
               sync_free=True)
     m = _model(params, **kw)
     bucket = m.enable_flat_grads()
-    eager = {}
+    eager, counts = {}, {}
     for i in (0, 1, 2, 4):  # also seeds the intersection-capacity statistics the capture needs
         bucket.zero_()
         ld = m.get_loss_dict(m.get_outputs(cams[i]), dict(batch))
         (ld["main_loss"] + ld["scale_reg"]).backward()
         eager[i] = (float(ld["main_loss"] + ld["scale_reg"]), bucket.flat.clone())
+        counts[i] = int(m.raster_out.info["n_isects_dev"])
     del ld  # a live autograd graph would pin AccumulateGrad nodes created on the default stream (see graph_step.py)
-    step = GraphedTrainStep(m, bucket, cams[0], batch, n_slots=2)
+    step = GraphedTrainStep(m, bucket, cams[0], batch, n_slots=2, capacity=capacity)
+    if capacity is not None:
+        assert min(counts.values()) > 2 * capacity, ("the test scene must overflow the captured capacity", counts)
+        worst = max(counts, key=counts.get)  # recapture() then has room for every view below
+        step(cams[worst], 0)
+        with pytest.raises(DnrCapacityError):
+            step.check_capacity(wait=True)
+        assert step.max_count == counts[worst]
+        step.recapture()
+        assert step.capacity > counts[worst]
     for i, slot in ((4, 0), (1, 1), (2, 0)):
         for k, v in batch.items():
             step.batches[slot][k].copy_(v)
         loss = step(cams[i], slot)
         torch.cuda.synchronize()
+        step.check_capacity(wait=True)
         assert abs(float(loss) - eager[i][0]) <= 1e-5 * max(1.0, abs(eager[i][0])), (i, float(loss), eager[i][0])
         rel = float((bucket.flat - eager[i][1]).norm() / (eager[i][1].norm() + 1e-30))
         assert rel < 1e-4, (i, rel)
