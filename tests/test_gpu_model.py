@@ -88,6 +88,68 @@ def test_loss_dict_matches_oracle_and_gradients_flow(depth_type):
     assert m.xys_flat.absgrad is not None and m.xys_flat.grad is not None
 
 
+def _fp64_oracle_loss(params, cam, batch, depth_type, ssim_lambda, **oracle_kw):
+    """The reference's loss for the same view in fp64: (1 - l) L1 + l (1 - SSIM) + DNRegularization, with the uint8 image
+    and normal maps read as value / 255 (the image clamped at 10/255 for the regulariser, quirk B10)."""
+    from dn_splatter_b200.dn_model import ssim
+    from oracle import dn_ref
+
+    p, ref = oracle_outputs(params, cam, dtype=torch.float64, requires_grad=True, **oracle_kw)
+    gt_img = batch["image"].double() / 255.0
+    loss = (1 - ssim_lambda) * (gt_img - ref["rgb"]).abs().mean()
+    if ssim_lambda > 0:
+        loss = loss + ssim_lambda * (1 - ssim(gt_img.permute(2, 0, 1)[None], ref["rgb"].permute(2, 0, 1)[None]))
+    loss = loss + dn_ref.dn_regularization(ref["depth"], batch["mono_depth"].double(), ref["normal"],
+                                           batch["normal"].double() / 255.0, p["scales"], gt_img.clamp(min=10 / 255.0),
+                                           depth_lambda=0.2, depth_loss_type=depth_type)
+    loss.backward()
+    return float(loss.detach()), p
+
+
+def _check_loss_dict_against_fp64_oracle(hw, depth_type, ssim_lambda, **cfg_kw):
+    from dn_splatter_b200.losses import DepthLossType
+
+    H, W = hw
+    params, cam = scene_and_camera(500, W, H, view=2)
+    g = torch.Generator().manual_seed(H * 100 + W)
+    depth = 2 + 6 * torch.rand(H, W, 1, generator=g)
+    depth[torch.rand(H, W, 1, generator=g) < 0.1] = 0.0
+    batch = {"image": (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8), "mono_depth": depth,
+             "normal": (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8)}
+    m = _model(params, use_depth_loss=True, depth_lambda=0.2, ssim_lambda=ssim_lambda,
+               depth_loss_type=DepthLossType(depth_type if depth_type != "MSE" else "mse"), **cfg_kw)
+    ld = m.get_loss_dict(m.get_outputs(_camera(cam)), {k: v.cuda() for k, v in batch.items()})
+    ld["main_loss"].backward()
+    want, p = _fp64_oracle_loss(params, cam, batch, depth_type, ssim_lambda,
+                                rasterize_mode=cfg_kw.get("rasterize_mode", "classic"))
+    assert abs(float(ld["main_loss"]) - want) <= 2e-4 * max(1.0, abs(want)), (float(ld["main_loss"]), want)
+    errs = {k: float((m.gauss_params[k].grad.cpu().double() - p[k].grad).norm() / p[k].grad.norm())
+            for k in ("means", "quats", "scales", "opacities", "features_dc", "features_rest")}
+    bad = {k: f"{v:.3e}" for k, v in errs.items() if not v <= 1e-3}
+    assert not bad, f"relative gradient error above 1e-3: {bad}"
+
+
+@needs_cuda
+@pytest.mark.parametrize("ssim_lambda", [0.0, 0.2])
+@pytest.mark.parametrize("depth_type", ["EdgeAwareLogL1", "LogL1", "L1", "MSE"])
+@pytest.mark.parametrize("hw", [(49, 81), (53, 75)], ids=["81x49", "75x53"])
+def test_loss_dict_gradients_match_fp64_oracle_at_ragged_sizes(hw, depth_type, ssim_lambda):
+    """get_loss_dict's gradients at frame sizes that are not multiples of the tile: the fused photometric loss
+    (FusedPhotometric with SSIM, or FusedL1) and the regularisers evaluated in raster_bwd's prologue read neighbours
+    through clamped indices along the ragged edge.  uint8 image and normal supervision."""
+    _check_loss_dict_against_fp64_oracle(hw, depth_type, ssim_lambda)
+
+
+@needs_cuda
+@pytest.mark.parametrize("ssim_lambda", [0.0, 0.2])
+@pytest.mark.parametrize("hw", [(49, 81), (80, 128)], ids=["81x49", "128x80"])
+def test_antialiased_two_pass_loss_dict_matches_fp64_oracle(hw, ssim_lambda):
+    """rasterize_mode="antialiased" with normals renders twice (colour / depth with opacity x compensation, normals
+    with the plain opacity) and sums both passes' gradients."""
+    _check_loss_dict_against_fp64_oracle(hw, "EdgeAwareLogL1", ssim_lambda, rasterize_mode="antialiased",
+                                         predict_normals=True)
+
+
 @needs_cuda
 def test_flat_grad_bucket_equals_autograd_path():
     params, cam = scene_and_camera(700, 96, 96, view=1)

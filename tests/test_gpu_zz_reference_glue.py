@@ -16,12 +16,8 @@ needs_cuda = pytest.mark.skipif(not torch.cuda.is_available(), reason="needs a C
 
 @needs_cuda
 @pytest.mark.parametrize("f", FILES, ids=[os.path.basename(f) for f in FILES])
-def test_model_matches_reference_glue_goldens(f, request):
+def test_model_matches_reference_glue_goldens(f):
     z = load(f)
-    if z["cfg"].get("rasterize_mode") == "antialiased":
-        # antialiased + normals renders twice (colour antialiased, normals classic) like the reference; that host path
-        # was added after round 1's last GPU run, so a failure here must not fail the suite yet
-        request.applymarker(pytest.mark.xfail(strict=False, reason="antialiased + normals two-pass path: first GPU run pending"))
     m, cam, batch = model_from_golden(z, device="cuda")
     if bool(z["eval"]):
         m.eval()

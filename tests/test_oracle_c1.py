@@ -70,3 +70,93 @@ def test_c1_oracle_fp64_gradient_matches_finite_differences(name, idx):
     h = 1e-5
     numeric = (f(h) - f(-h)) / (2 * h)
     assert abs(analytic - numeric) <= 1e-4 * max(1.0, abs(numeric)) + 1e-6, (analytic, numeric)
+
+
+def _fd_check(params, cam, name, gi, comp, h=1e-5, **kw):
+    """fp64 autograd of the oracle vs a central difference, for parameter entry params[name][(gi,) + comp]; the
+    objective weights every output (rgb, covered depth, alpha, and the normal image except for `means`, quirk B3)."""
+    H, W = cam["height"], cam["width"]
+    _, probe = oracle_outputs(params, cam, dtype=torch.float64, **kw)
+    w = torch.rand(H, W, 3, generator=torch.Generator().manual_seed(1)).double()
+    covered = (probe["accumulation"] > 0).double()
+    with_normal = name != "means"
+
+    def total(o):
+        t = (o["rgb"] * w).sum() + 0.1 * (o["depth"] * covered).sum() + o["accumulation"].sum()
+        return t + (o["normal"] * w).sum() if with_normal else t
+
+    def f(delta):
+        q = {k: v.clone().double() for k, v in params.items()}
+        q[name][(gi,) + comp] += delta
+        return float(total(oracle_outputs(q, cam, dtype=torch.float64, **kw)[1]))
+
+    p, o = oracle_outputs(params, cam, dtype=torch.float64, requires_grad=True, **kw)
+    total(o).backward()
+    analytic = float(p[name].grad[(gi,) + comp])
+    numeric = (f(h) - f(-h)) / (2 * h)
+    assert numeric != 0.0, "the entry must influence the objective"
+    assert abs(analytic - numeric) <= 1e-4 * max(1.0, abs(numeric)) + 1e-6, (analytic, numeric)
+
+
+def _visible(params, cam, k, **kw):
+    _, probe = oracle_outputs(params, cam, dtype=torch.float64, **kw)
+    vis = torch.nonzero(probe["info"]["radii"] > 0).flatten()
+    return int(vis[k % len(vis)])
+
+
+@pytest.mark.parametrize("name,k,comp", [("opacities", 7, (0,)), ("scales", 3, (1,)), ("quats", 10, (2,)), ("quats", 4, (0,))])
+def test_oracle_antialiased_gradient_matches_finite_differences(name, k, comp):
+    """rasterize_mode="antialiased": opacity x compensation, compensation = sqrt(det(cov) / det(cov + 0.3 I))."""
+    params, cam = scene_and_camera(60, 48, 40, view=2)
+    gi = _visible(params, cam, k, rasterize_mode="antialiased")
+    _fd_check(params, cam, name, gi, comp, rasterize_mode="antialiased")
+
+
+@pytest.mark.parametrize("degree", [1, 2])
+@pytest.mark.parametrize("name", ["means", "features_rest"])
+def test_oracle_low_sh_degree_gradient_matches_finite_differences(degree, name):
+    """Active SH degree 1 and 2 with all 16 bases stored (the first 3000 training steps)."""
+    params, cam = scene_and_camera(60, 48, 40, view=2)
+    gi = _visible(params, cam, 5, sh_degree=degree)
+    comp = (1,) if name == "means" else ((degree + 1) ** 2 - 2, 0)  # the highest active basis
+    _fd_check(params, cam, name, gi, comp, sh_degree=degree)
+
+
+def test_oracle_opacity_gradient_of_alpha_clamped_gaussian_matches_finite_differences():
+    """The nearest visible Gaussian, moved to project onto a pixel centre at opacity 0.9995: its alpha clamps to 0.999
+    at that pixel (no opacity gradient there) and not elsewhere.  The step is chosen so that no pixel's opacity x vis
+    crosses 0.999 or 1/255."""
+    from oracle import dn_ref, gsplat_ref as G
+
+    params, cam = scene_and_camera(60, 48, 40, view=2)
+    _, probe = oracle_outputs(params, cam, dtype=torch.float64)
+    info = probe["info"]
+    vis = torch.nonzero(info["radii"] > 0).flatten()
+    gi = int(vis[torch.argmin(info["depths"][vis])])
+    vm = dn_ref.get_viewmat(cam["c2w"].double())
+    xc = params["means"][gi].double() @ vm[:3, :3].T + vm[:3, 3]
+    u = (cam["fx"] * xc[0] / xc[2] + cam["cx"]).clamp(1, cam["width"] - 2)
+    v = (cam["fy"] * xc[1] / xc[2] + cam["cy"]).clamp(1, cam["height"] - 2)
+    xc[0] = (u.floor() + 0.5 - cam["cx"]) * xc[2] / cam["fx"]
+    xc[1] = (v.floor() + 0.5 - cam["cy"]) * xc[2] / cam["fy"]
+    params = {k: t.clone() for k, t in params.items()}
+    params["means"][gi] = ((xc - vm[:3, 3]) @ vm[:3, :3]).float()
+    op = 0.9995
+    params["opacities"][gi] = torch.logit(torch.tensor(op, dtype=torch.float64)).float()
+    op = float(torch.sigmoid(params["opacities"][gi].double()))
+    # opacity x vis of this Gaussian at every pixel centre
+    _, probe = oracle_outputs(params, cam, dtype=torch.float64)
+    info = probe["info"]
+    ys, xs = torch.meshgrid(torch.arange(cam["height"], dtype=torch.float64) + 0.5,
+                            torch.arange(cam["width"], dtype=torch.float64) + 0.5, indexing="ij")
+    dx, dy = info["means2d"][gi, 0] - xs, info["means2d"][gi, 1] - ys
+    a, b, c = info["conics"][gi]
+    ov = op * torch.exp(-(0.5 * (a * dx * dx + c * dy * dy) + b * dx * dy))
+    centre = (int(info["means2d"][gi, 1]), int(info["means2d"][gi, 0]))
+    assert float(ov[centre]) > G.ALPHA_MAX, "the centre pixel must clamp"
+    assert float(probe["accumulation"][centre]) >= G.ALPHA_MAX, "the centre pixel must composite the clamped alpha"
+    # d(ov) = ov (1 - op) d(logit): keep it well inside the distance to both kinks
+    margin = float(torch.minimum((ov - G.ALPHA_MAX).abs(), (ov - G.ALPHA_MIN).abs()).min())
+    h = min(1e-5, 0.1 * margin / (1.0 - op))
+    assert h >= 1e-8, f"a pixel sits {margin:.2e} from a kink: no usable step"
+    _fd_check(params, cam, "opacities", gi, (0,), h=h)
