@@ -13,6 +13,7 @@ FLAG_ACTIVATED, FLAG_ANTIALIASED, FLAG_NORMALS, FLAG_ACCUMULATE, FLAG_EXACT_LIST
 FLAG_HOST_CAMERA = 32
 FLAG_COMPACT_BWD = 64
 FLAG_TOUCHED_BWD = 128
+FLAG_PERSISTENT_WS = 256
 LOSS_FUSED_BWD, LOSS_IMG_U8, LOSS_NORMAL_U8, LOSS_EDGE_FROM_IMAGE = 1, 2, 4, 8
 REC_FLOATS, REC_FLOATS_N, GRAD_FLOATS = 12, 16, 16
 DEPTH_LOSS_TYPES = {None: 0, "EdgeAwareLogL1": 1, "LogL1": 2, "L1": 3, "MSE": 4}
@@ -54,6 +55,12 @@ class DnrAdamSeg(C.Structure):
                 ("bc1", C.c_double), ("bc2_sqrt", C.c_double), ("dense", C.c_int64)]
 
 
+class DnrGradSeg(C.Structure):
+    """Mirror of struct DnrGradSeg (include/dnr.h)."""
+
+    _fields_ = [("g", _p), ("width", _i), ("dense", _i)]
+
+
 PEER_MAX = 8
 
 
@@ -81,6 +88,7 @@ KERNELS_PER_CALL = {
     "dnr_loss_fwd": (2, 0), "dnr_loss_bwd": (1, 0), "dnr_scale_loss_fwd": (1, 0), "dnr_scale_loss_bwd": (1, 0),
     "dnr_l1_fwd": (1, 0), "dnr_l1_bwd": (1, 0), "dnr_u8_to_f32": (1, 0),
     "dnr_ssim_fwd": (1, 0), "dnr_ssim_bwd": (1, 0), "dnr_ssim_fwd_ex": (1, 0), "dnr_ssim_bwd_ex": (1, 0), "dnr_photometric_fwd": (2, 0), "dnr_photometric_bwd": (1, 0), "dnr_adam_step": (1, 0), "dnr_adam_step_reduce": (2, 0),
+    "dnr_grad_zero": (1, 0),
     "dnr_knn_build": (2, 1), "dnr_knn_query": (1, 0), "dnr_density": (1, 0), "dnr_ray_densities": (1, 0),
 }
 LAUNCHES = {"handwritten": 0, "cub": 0}
@@ -179,6 +187,8 @@ def load():
     lib.dnr_adam_step.argtypes = [C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_void_p]
     lib.dnr_adam_step_reduce.restype = C.c_int
     lib.dnr_adam_step_reduce.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_double, C.c_double, C.c_void_p, C.c_void_p]
+    lib.dnr_grad_zero.restype = C.c_int
+    lib.dnr_grad_zero.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int32, C.c_void_p]
     lib.dnr_knn_workspace_bytes.restype = C.c_int64
     lib.dnr_knn_workspace_bytes.argtypes = [C.c_int32, C.c_void_p]
     lib.dnr_knn_build.restype = C.c_int
@@ -209,7 +219,7 @@ EXPORTS = (
     "dnr_version", "dnr_error_string", "dnr_project_fwd", "dnr_bin_scan_workspace_bytes", "dnr_bin_scan",
     "dnr_bin_sort_workspace_bytes", "dnr_bin_sort", "dnr_depth_order_ptr", "dnr_raster_fwd", "dnr_finalize_fwd", "dnr_normal_from_depth",
     "dnr_raster_bwd", "dnr_project_bwd", "dnr_loss_fwd", "dnr_loss_bwd", "dnr_scale_loss_fwd", "dnr_scale_loss_bwd",
-    "dnr_l1_fwd", "dnr_l1_bwd", "dnr_u8_to_f32", "dnr_ssim_fwd", "dnr_ssim_bwd", "dnr_ssim_fwd_ex", "dnr_ssim_bwd_ex", "dnr_photometric_fwd", "dnr_photometric_bwd", "dnr_adam_step", "dnr_adam_step_reduce", "dnr_knn_workspace_bytes", "dnr_knn_build", "dnr_knn_query",
+    "dnr_l1_fwd", "dnr_l1_bwd", "dnr_u8_to_f32", "dnr_ssim_fwd", "dnr_ssim_bwd", "dnr_ssim_fwd_ex", "dnr_ssim_bwd_ex", "dnr_photometric_fwd", "dnr_photometric_bwd", "dnr_adam_step", "dnr_adam_step_reduce", "dnr_grad_zero", "dnr_knn_workspace_bytes", "dnr_knn_build", "dnr_knn_query",
     "dnr_density", "dnr_ray_densities",
 )
 

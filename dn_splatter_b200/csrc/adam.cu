@@ -1,8 +1,10 @@
 // One-launch Adam over every Gaussian parameter group (SURVEY.md §8f-3, "next" row).  The reference builds one
 // torch.optim.Adam per group (/root/reference/dn_splatter/dn_config.py:29-68: lr per group, eps 1e-15, no weight decay,
 // no amsgrad) and nerfstudio steps them one after the other [EXT Optimizers.optimizer_step]; at 1M Gaussians that is
-// 62M parameters x 28 B = 1.7 GB of HBM traffic, i.e. ~0.25 ms at speed of light, but 7 optimizers x several
-// elementwise passes each in torch.  Here: one kernel, blockIdx.y = group, float4 grid-stride over the group.
+// 59M parameters x 28 B = 1.65 GB of HBM traffic (at least 0.49 ms at the H100 SXM data sheet's 3.35 TB/s), but
+// 7 optimizers x several elementwise passes each in torch.  Here: one kernel, blockIdx.y = group, float4 grid-stride
+// over the group.  A single-GPU bucket whose `touched` flags are valid is stepped by adam_reduce_kernel<1> instead, which
+// reads only the touched gradient rows (28 B -> ~24.4 B per float).
 //
 // Update rule — torch.optim.Adam [EXT torch 2.x, _single_tensor_adam], dense (zero-gradient rows still decay):
 //   m = m + (1-b1)(g - m)  [lerp];  v = b2 v + (1-b2) g g;  p -= (lr / bc1) * m / (sqrt(v) / sqrt(bc2) + eps)
@@ -108,8 +110,11 @@ struct AdamReduceLaunch {
 // WORLD = the rank count rounded up to 2 / 4 / 8: the peer loop unrolls completely, every peer's float4 is requested with
 // a predicated load BEFORE the first one is consumed (a thread otherwise pays one NVLink round trip, ~2 us, per touching
 // rank in turn), and the local p / m / v loads are already in flight behind them.  Bits of ranks >= world are never set.
+// WORLD = 1 is the single-GPU step over a bucket with valid flags: the mask is the bucket's own `touched` array, so the
+// gradient rows of untouched Gaussians (~90 % of the bucket) are never read; p / m / v are still read and written for
+// every element, and g = 0 rows still decay, exactly as in adam_kernel.
 template <int WORLD>
-__global__ void __launch_bounds__(256, WORLD > 4 ? 3 : 4) adam_reduce_kernel(const AdamReduceLaunch L, const PeerDev P, const uint8_t* __restrict__ mask) {
+__global__ void __launch_bounds__(256, WORLD > 4 ? 3 : (WORLD > 1 ? 4 : 5)) adam_reduce_kernel(const AdamReduceLaunch L, const PeerDev P, const uint8_t* __restrict__ mask) {
   const AdamSegDev& s = L.adam.seg[blockIdx.y];
   const float w1 = L.adam.w1, b2 = L.adam.beta2, w2 = L.adam.w2;
   const float step_size = s.step_size, bc2_sqrt = s.bc2_sqrt, eps = s.eps;
@@ -126,8 +131,9 @@ __global__ void __launch_bounds__(256, WORLD > 4 ? 3 : 4) adam_reduce_kernel(con
     // covers (up to four of them when width == 1) only decides which peers are worth reading; the sum runs in rank order
     // on every replica.  n < 2^32 (checked by the host): 32-bit divisions.
     const uint32_t e = (uint32_t)(i << 2);
-    const uint32_t mk = all_ranks | (uint32_t)mask[e / width] | (uint32_t)mask[(e + 1u) / width] |
-                        (uint32_t)mask[(e + 2u) / width] | (uint32_t)mask[(e + 3u) / width];
+    uint32_t mk = all_ranks | (uint32_t)mask[e / width] | (uint32_t)mask[(e + 1u) / width] |
+                  (uint32_t)mask[(e + 2u) / width] | (uint32_t)mask[(e + 3u) / width];
+    if (WORLD == 1) mk = mk != 0u;  // touched flags: any non-zero byte
     float4 p = p4[i], m = m4[i], v = v4[i];
     float4 t[WORLD];
 #pragma unroll
@@ -147,7 +153,8 @@ __global__ void __launch_bounds__(256, WORLD > 4 ? 3 : 4) adam_reduce_kernel(con
     p4[i] = p; m4[i] = m; v4[i] = v;
   }
   for (int64_t i = (n4 << 2) + tid; i < n; i += stride) {  // tail
-    const uint32_t mk = all_ranks | (uint32_t)mask[(uint32_t)i / width];
+    uint32_t mk = all_ranks | (uint32_t)mask[(uint32_t)i / width];
+    if (WORLD == 1) mk = mk != 0u;
     float g = 0.f;
     for (int k = 0; k < P.world; ++k)
       if ((mk >> k) & 1u) g += P.flat[k][off + i];
@@ -155,6 +162,46 @@ __global__ void __launch_bounds__(256, WORLD > 4 ? 3 : 4) adam_reduce_kernel(con
     adam_one(p, g, m, v, w1, b2, w2, step_size, bc2_sqrt, eps);
     s.p[i] = p; s.m[i] = m; s.v[i] = v;
   }
+}
+
+struct GradZeroLaunch {
+  float* g[DNR_ADAM_MAX_SEGS];
+  int32_t width[DNR_ADAM_MAX_SEGS];
+  int32_t dense[DNR_ADAM_MAX_SEGS];
+  int n_segs;
+};
+
+// dnr_grad_zero: a CTA owns GZ_CHUNK consecutive Gaussians.  It reads their flags once, zeroes the float4s of each segment
+// that hold a flagged Gaussian's row (all of them in a dense segment; the untouched elements a float4 shares with a flagged
+// row are zero already), and only then clears the flags it read: no other CTA reads them, so there is no race.
+// GZ_CHUNK is a multiple of 4, so every chunk of every segment starts on a float4.
+constexpr int GZ_CHUNK = 256;
+
+__global__ void __launch_bounds__(GZ_CHUNK) grad_zero_kernel(const GradZeroLaunch L, uint8_t* __restrict__ touched, int n) {
+  __shared__ uint8_t s_f[GZ_CHUNK];
+  const int tid = threadIdx.x;
+  const int g0 = blockIdx.x * GZ_CHUNK;
+  const int ng = min(GZ_CHUNK, n - g0);
+  const uint8_t f = tid < ng ? touched[g0 + tid] : 0;
+  s_f[tid] = f;
+  const bool any = __syncthreads_or(f != 0);
+  const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+  for (int s = 0; s < L.n_segs; ++s) {
+    const bool dense = L.dense[s] != 0;
+    if (!dense && !any) continue;
+    const uint32_t w = (uint32_t)L.width[s];
+    float4* out = reinterpret_cast<float4*>(L.g[s] + (size_t)g0 * w);
+    const uint32_t n4 = ((uint32_t)ng * w + 3u) >> 2;  // the last chunk may write into the segment's zero padding
+    for (uint32_t i = tid; i < n4; i += GZ_CHUNK) {
+      bool hit = dense;
+      if (!dense) {
+        const uint32_t last = min((4u * i + 3u) / w, (uint32_t)ng - 1u);
+        for (uint32_t j = (4u * i) / w; j <= last; ++j) hit |= s_f[j] != 0;
+      }
+      if (hit) out[i] = z;
+    }
+  }
+  if (f) touched[g0 + tid] = 0;
 }
 
 }  // namespace
@@ -180,7 +227,7 @@ extern "C" int dnr_adam_step_reduce(const DnrAdamSeg* segs, const int32_t* width
   if (n_segs <= 0 || n_segs > DNR_ADAM_MAX_SEGS) return DNR_E_SIZE;
   if (peers->world < 1 || peers->world > DNR_PEER_MAX || peers->rank < 0 || peers->rank >= peers->world || peers->n_gauss <= 0)
     return DNR_E_SIZE;
-  if (!peers->mask) return DNR_E_NULL;
+  if (!peers->mask && peers->world > 1) return DNR_E_NULL;
   AdamReduceLaunch L;
   int64_t longest = 0;
   if (const int rc = fill_adam_launch(segs, n_segs, beta1, beta2, L.adam, longest)) return rc;
@@ -203,13 +250,16 @@ extern "C" int dnr_adam_step_reduce(const DnrAdamSeg* segs, const int32_t* width
   }
   cudaStream_t s = (cudaStream_t)stream;
   const int n = peers->n_gauss;
-  peer_mask_kernel<<<(n / 16 + 256) / 256, 256, 0, s>>>(P, n, peers->mask);
-  DNR_CHECK_LAUNCH();
+  if (peers->world > 1) {
+    peer_mask_kernel<<<(n / 16 + 256) / 256, 256, 0, s>>>(P, n, peers->mask);
+    DNR_CHECK_LAUNCH();
+  }
   int64_t blocks = (longest / 4 + 255) / 256;
   if (blocks > DNR_NUM_SMS * 8) blocks = DNR_NUM_SMS * 8;
   if (blocks < 1) blocks = 1;
   const dim3 grid((unsigned)blocks, (unsigned)n_segs);
-  if (peers->world <= 2) adam_reduce_kernel<2><<<grid, 256, 0, s>>>(L, P, peers->mask);
+  if (peers->world == 1) adam_reduce_kernel<1><<<grid, 256, 0, s>>>(L, P, P.touched[0]);
+  else if (peers->world <= 2) adam_reduce_kernel<2><<<grid, 256, 0, s>>>(L, P, peers->mask);
   else if (peers->world <= 4) adam_reduce_kernel<4><<<grid, 256, 0, s>>>(L, P, peers->mask);
   else adam_reduce_kernel<8><<<grid, 256, 0, s>>>(L, P, peers->mask);
   DNR_CHECK_LAUNCH();
@@ -227,6 +277,23 @@ extern "C" int dnr_adam_step(const DnrAdamSeg* segs, int32_t n_segs, double beta
   if (blocks > DNR_NUM_SMS * 8) blocks = DNR_NUM_SMS * 8;
   if (blocks < 1) blocks = 1;
   adam_kernel<<<dim3((unsigned)blocks, (unsigned)n_segs), 256, 0, (cudaStream_t)stream>>>(L);
+  DNR_CHECK_LAUNCH();
+  return 0;
+}
+
+extern "C" int dnr_grad_zero(const DnrGradSeg* segs, int32_t n_segs, uint8_t* touched, int32_t n_gauss, void* stream) {
+  if (!segs || !touched) return DNR_E_NULL;
+  if (n_segs <= 0 || n_segs > DNR_ADAM_MAX_SEGS || n_gauss <= 0) return DNR_E_SIZE;
+  GradZeroLaunch L;
+  L.n_segs = n_segs;
+  for (int i = 0; i < n_segs; ++i) {
+    if (!segs[i].g) return DNR_E_NULL;
+    if (segs[i].width <= 0 || segs[i].width > 4096 || ((uintptr_t)segs[i].g & 15)) return DNR_E_SIZE;
+    L.g[i] = segs[i].g;
+    L.width[i] = segs[i].width;
+    L.dense[i] = segs[i].dense;
+  }
+  grad_zero_kernel<<<(n_gauss + GZ_CHUNK - 1) / GZ_CHUNK, GZ_CHUNK, 0, (cudaStream_t)stream>>>(L, touched, n_gauss);
   DNR_CHECK_LAUNCH();
   return 0;
 }

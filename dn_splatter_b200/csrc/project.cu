@@ -687,6 +687,11 @@ __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_touched_kernel(cons
       for (int k = 0; k < 3; ++k) { a.v_means[i * 3 + k] += vm[k]; a.v_scales[i * 3 + k] += vs[k]; a.v_sh_dc[i * 3 + k] += vdc[k]; }
       for (int k = 0; k < 4; ++k) a.v_quats[i * 4 + k] += vq[k];
       a.v_opacities[i] += vo;
+      // the record is consumed: leave grad_records all zero for the next dnr_raster_bwd (DNR_FLAG_PERSISTENT_WS), 64 B
+      // per touched Gaussian instead of a memset of the whole buffer
+      float4* gr = reinterpret_cast<float4*>(a.grad_records + (size_t)i * DNR_GRAD_FLOATS);
+      const float4 z = make_float4(0.f, 0.f, 0.f, 0.f);
+      gr[0] = z; gr[1] = z; gr[2] = z; gr[3] = z;
     }
     __syncthreads();
     if (nrest > 0) {

@@ -686,8 +686,12 @@ extern "C" int dnr_raster_bwd(const DnrArgs* a, void* stream) {
     if (a->use_normal_loss && (!normals || !a->gt_normal)) return DNR_E_NULL;
   }
   cudaStream_t s = (cudaStream_t)stream;
-  DNR_CUDA(cudaMemsetAsync(a->grad_records, 0, (size_t)a->n_gauss * DNR_GRAD_FLOATS * sizeof(float), s));
-  if (a->touched) DNR_CUDA(cudaMemsetAsync(a->touched, 0, (size_t)a->n_gauss, s));
+  if (a->flags & DNR_FLAG_PERSISTENT_WS) {
+    if (!a->touched) return DNR_E_NULL;  // the flags are what lets the next project_bwd restore grad_records to zero
+  } else {
+    DNR_CUDA(cudaMemsetAsync(a->grad_records, 0, (size_t)a->n_gauss * DNR_GRAD_FLOATS * sizeof(float), s));
+    if (a->touched) DNR_CUDA(cudaMemsetAsync(a->touched, 0, (size_t)a->n_gauss, s));
+  }
   if (a->n_isects == 0) return 0;
   const dim3 grid(dnr_tiles_x(a), dnr_tiles_y(a));
   const int sx = dnr_stiles_x(a);

@@ -236,6 +236,8 @@ class DNSplatterModel(_ModelBase):
                                       "`scales` segment (min-scale regulariser); other parameter-only loss terms make more "
                                       "segments dense: use peer=False (NCCL all-reduce)")
         self._bucket = PeerGradBucket(dict(self.gauss_params), group=group) if peer else FlatGradBucket(dict(self.gauss_params))
+        if self.config.use_scale_regularization or self.config.use_sparse_loss:
+            self._bucket.sparse_ok = False  # the same parameter-only terms: no sparse zero_() / Adam reads
         self._bucket_mode = (bool(peer), group)  # densification re-creates the bucket in the same mode (densify._replace_params)
         return self._bucket
 

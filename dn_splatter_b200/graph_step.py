@@ -134,7 +134,7 @@ class GraphedTrainStep:
         m = self.model
         m.__dict__["_graph_cam"] = self.cam
         try:
-            self.bucket.flat.zero_()
+            self.bucket.zero_()  # sparse or dense as the bucket's flags allow when the graph is captured
             L.capture_ok("bucket zero")
             out = m.get_outputs(self._camera)
             L.capture_ok("get_outputs")

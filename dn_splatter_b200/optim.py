@@ -7,9 +7,12 @@ learning rate per group, eps 1e-15, an exponential schedule on `means`) and nerf
 checkpointing work unchanged — but `step()` is a single `dnr_adam_step` launch over all groups.
 
 The update rule is pinned against torch.optim.Adam on the CPU through `reference_step` (tests/test_fused_adam_cpu.py)
-and the kernel against torch.optim.Adam on the GPU (tests/test_gpu_model.py); it runs at the HBM roofline (0.27 ms for
-59 M floats).  `step_reduce(bucket)` is the multi-GPU form: the gradient sum over ranks happens inside the same kernel,
-read from the peers' buckets over NVLink (parallel.PeerGradBucket, tests/test_gpu_multi.py).
+and the kernel against torch.optim.Adam on the GPU (tests/test_gpu_model.py).  The dense pass moves 28 B per float
+(1.65 GB for 59 M floats: at least 0.49 ms at the H100 SXM data sheet's 3.35 TB/s).  When the gradients are views of a
+parallel.FlatGradBucket whose `touched` flags are valid, `step()` reads only the flagged gradient rows (plus the dense
+`scales` segment) through dnr_adam_step_reduce at world 1; results are bit-identical, because the other rows are exactly
+zero.  `step_reduce(bucket)` is the multi-GPU form: the gradient sum over ranks happens inside the same kernel, read from
+the peers' buckets over NVLink (parallel.PeerGradBucket, tests/test_gpu_multi.py).
 """
 from __future__ import annotations
 
@@ -20,6 +23,7 @@ from typing import Dict, Iterable, Optional
 import torch
 
 from . import _lib as L
+from .rasterize import _timed
 
 
 def bias_corrections(step: int, beta1: float, beta2: float):
@@ -80,6 +84,13 @@ class FusedAdam(torch.optim.Optimizer):
             raise L.DnrError("FusedAdam needs CUDA parameters (no CPU path)")
         b1, b2 = segs[0][8], segs[0][9]
         assert all(s[8] == b1 and s[9] == b2 for s in segs), "one (beta1, beta2) pair per launch"
+        bucket = self._flagged_bucket(segs)
+        if bucket is not None:  # sparse gradient reads: the bucket's own flags are the mask, no peers, no barriers
+            pr = L.DnrPeerReduce()
+            pr.world, pr.rank, pr.n_gauss = 1, 0, bucket.n_gauss
+            pr.peer_flat[0], pr.peer_touched[0] = bucket.flat.data_ptr(), bucket.touched.data_ptr()
+            _timed("adam", self._launch_reduce, segs, bucket, pr)
+            return loss
         arr = (L.DnrAdamSeg * len(segs))()
         for i, (p, g, m, v, lr, eps, bc1, bc2s, _, _) in enumerate(segs):
             assert p.is_contiguous() and g.is_contiguous() and m.is_contiguous() and v.is_contiguous()
@@ -87,8 +98,24 @@ class FusedAdam(torch.optim.Optimizer):
             arr[i].p, arr[i].g, arr[i].m, arr[i].v = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
             arr[i].n, arr[i].lr, arr[i].eps, arr[i].bc1, arr[i].bc2_sqrt = p.numel(), lr, eps, bc1, bc2s
         stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
-        L.check(L.load().dnr_adam_step(ctypes.cast(arr, ctypes.c_void_p), len(segs), b1, b2, stream), "dnr_adam_step")
+        L.check(_timed("adam", L.load().dnr_adam_step, ctypes.cast(arr, ctypes.c_void_p), len(segs), b1, b2, stream),
+                "dnr_adam_step")
         return loss
+
+    @staticmethod
+    def _flagged_bucket(segs):
+        """The FlatGradBucket that every gradient of `segs` is a segment of, if its flags are valid; else None."""
+        from .parallel import bucket_of
+
+        bucket = bucket_of(segs[0][1])
+        if bucket is None or not bucket.flags_valid:
+            return None
+        views = {v.data_ptr(): n for n, v in bucket.views.items()}
+        for p, g, *_ in segs:
+            name = views.get(g.data_ptr())
+            if name is None or bucket.params[name] is not p:
+                return None
+        return bucket
 
     @torch.no_grad()
     def step_reduce(self, bucket):
@@ -98,27 +125,32 @@ class FusedAdam(torch.optim.Optimizer):
         segs = self._segments()
         if not segs:
             return
-        b1, b2 = segs[0][8], segs[0][9]
-        arr = (L.DnrAdamSeg * len(segs))()
-        widths = (ctypes.c_int32 * len(segs))()
-        lo, hi = bucket.flat.data_ptr(), bucket.flat.data_ptr() + bucket.flat.numel() * 4
-        for i, (p, g, m, v, lr, eps, bc1, bc2s, _, _) in enumerate(segs):
-            assert lo <= g.data_ptr() < hi, "parameter gradients must be views of the peer bucket"
-            assert p.is_contiguous() and m.is_contiguous() and v.is_contiguous() and p.shape[0] == bucket.n_gauss
-            arr[i].p, arr[i].g, arr[i].m, arr[i].v = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
-            arr[i].n, arr[i].lr, arr[i].eps, arr[i].bc1, arr[i].bc2_sqrt = p.numel(), lr, eps, bc1, bc2s
-            widths[i] = p.numel() // bucket.n_gauss
-            arr[i].dense = int(any(bucket.params[name] is p for name in bucket.dense_params))
         pr = L.DnrPeerReduce()
         pr.world, pr.rank, pr.n_gauss = bucket.world, bucket.rank, bucket.n_gauss
         for k in range(bucket.world):
             pr.peer_flat[k], pr.peer_touched[k] = bucket.peer_flat[k], bucket.peer_touched[k]
         pr.mask = bucket.mask.data_ptr()
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         bucket.barrier()  # every rank's backward has finished writing its bucket and flags
+        self._launch_reduce(segs, bucket, pr)
+        bucket.barrier()  # nobody zeroes its bucket while a peer still reads it
+
+    @staticmethod
+    def _launch_reduce(segs, bucket, pr) -> None:
+        """dnr_adam_step_reduce over `segs`, whose gradients are segments of `bucket` (`pr`: the ranks' buckets and flags)."""
+        b1, b2 = segs[0][8], segs[0][9]
+        arr = (L.DnrAdamSeg * len(segs))()
+        widths = (ctypes.c_int32 * len(segs))()
+        lo, hi = bucket.flat.data_ptr(), bucket.flat.data_ptr() + bucket.flat.numel() * 4
+        for i, (p, g, m, v, lr, eps, bc1, bc2s, _, _) in enumerate(segs):
+            assert lo <= g.data_ptr() < hi, "parameter gradients must be views of the bucket"
+            assert p.is_contiguous() and m.is_contiguous() and v.is_contiguous() and p.shape[0] == bucket.n_gauss
+            arr[i].p, arr[i].g, arr[i].m, arr[i].v = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
+            arr[i].n, arr[i].lr, arr[i].eps, arr[i].bc1, arr[i].bc2_sqrt = p.numel(), lr, eps, bc1, bc2s
+            widths[i] = p.numel() // bucket.n_gauss
+            arr[i].dense = int(any(bucket.params[name] is p for name in bucket.dense_params))
+        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
         L.check(L.load().dnr_adam_step_reduce(ctypes.cast(arr, ctypes.c_void_p), ctypes.cast(widths, ctypes.c_void_p), len(segs),
                                               b1, b2, ctypes.byref(pr), stream), "dnr_adam_step_reduce")
-        bucket.barrier()  # nobody zeroes its bucket while a peer still reads it
 
     @torch.no_grad()
     def reference_step(self):

@@ -7,6 +7,8 @@ The reference only wraps the model in DDP(find_unused_parameters=True) (dn_pipel
 cope with densification re-creating parameters; this module is the working equivalent for the hot path."""
 from __future__ import annotations
 
+import ctypes
+import weakref
 from typing import Dict, Iterable, List, Optional
 
 import torch
@@ -15,11 +17,25 @@ from torch import Tensor
 
 GRAD_PARAMS = ("means", "scales", "quats", "features_dc", "features_rest", "opacities")
 
+_BUCKETS: "weakref.WeakValueDictionary[int, FlatGradBucket]" = weakref.WeakValueDictionary()  # by flat.data_ptr()
+
+
+def bucket_of(grad: Tensor) -> Optional["FlatGradBucket"]:
+    """The live FlatGradBucket that `grad` is a view of, or None."""
+    base = grad._base
+    b = _BUCKETS.get(base.data_ptr()) if base is not None else None
+    return b if b is not None and b.flat.data_ptr() == base.data_ptr() and b.flat.numel() == base.numel() else None
+
 
 class FlatGradBucket:
     """One contiguous fp32 buffer holding the gradients of the six optimised gauss_params (59 floats per
     Gaussian at SH degree 3); `param.grad` are views into it, so autograd, the rasterizer's grad-sink path
-    and the all-reduce all touch the same memory."""
+    and the all-reduce all touch the same memory.
+
+    The bucket also owns the rasterizer's per-Gaussian `touched` flags and its always-zero `grad_records` workspace
+    (DNR_FLAG_PERSISTENT_WS).  The flags accumulate over every backward since the last `zero_()`.  While they cover every
+    non-zero row (`flags_valid`), `zero_()` clears only the flagged rows and FusedAdam.step() reads only the flagged
+    gradient rows: about 10 % of the bucket at 1 M Gaussians / 1080p."""
 
     def __init__(self, params: Dict[str, torch.nn.Parameter], names: Iterable[str] = GRAD_PARAMS):
         self.names = [n for n in names if n in params]
@@ -34,6 +50,18 @@ class FlatGradBucket:
             p.grad = v
             self.views[n] = v
             off += self._padded(p.numel())
+        self.n_gauss = next(iter(self.params.values())).shape[0]
+        self.touched = torch.zeros(self.n_gauss, dtype=torch.uint8, device=dev)
+        self.grad_records = torch.zeros(self.n_gauss, 16, dtype=torch.float32, device=dev)  # DNR_GRAD_FLOATS
+        # parameters whose gradient is non-zero for every Gaussian (a loss term that depends on the parameters alone:
+        # DNRegularization's min-scale term on `scales`): never covered by the flags, zeroed and read in full
+        self.dense_params = {"scales"} & set(self.params)
+        # False for configs with other parameter-only loss terms (dn_model.enable_flat_grads)
+        self.sparse_ok = True
+        # flags_valid: every non-zero row outside the dense segments is flagged.  Only a flagged backward through sink()
+        # makes the flags valid; a fresh bucket may have been filled by other means.
+        self.flags_valid, self._clean = False, False
+        _BUCKETS[self.flat.data_ptr()] = self
 
     @staticmethod
     def _padded(n: int) -> int:
@@ -41,14 +69,34 @@ class FlatGradBucket:
         return (n + 3) & ~3
 
     def zero_(self) -> None:
-        self.flat.zero_()
+        if self.flags_valid:
+            from . import _lib as L
+            from .rasterize import _timed
+
+            segs = (L.DnrGradSeg * len(self.names))()
+            for i, n in enumerate(self.names):
+                v = self.views[n]
+                segs[i].g, segs[i].width, segs[i].dense = v.data_ptr(), v.numel() // self.n_gauss, int(n in self.dense_params)
+            stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+            L.check(_timed("bucket_zero", L.load().dnr_grad_zero, ctypes.cast(segs, ctypes.c_void_p), len(segs),
+                           self.touched.data_ptr(), self.n_gauss, stream), "dnr_grad_zero")
+        else:
+            self.flat.zero_()
+            self.touched.zero_()
+        self.flags_valid, self._clean = False, True
         for n, p in self.params.items():  # re-attach in case an optimizer set .grad = None
             if p.grad is None or p.grad.data_ptr() != self.views[n].data_ptr():
                 p.grad = self.views[n]
 
+    def note_backward(self, flagged: bool) -> None:
+        """Called by the rasterizer's backward after it wrote into sink(): `flagged` = it set the flag of every row it
+        wrote.  The flags stay valid only while every such backward since the last zero_() was flagged."""
+        self.flags_valid = flagged and self.sparse_ok and (self.flags_valid or self._clean)
+        self._clean = False
+
     def sink(self) -> Dict[str, Tensor]:
         """Buffers for dn_rasterize(grad_sink=...)."""
-        return self.views
+        return dict(self.views, touched=self.touched, grad_records=self.grad_records, bucket=self)
 
     def all_reduce(self, group=None, async_op: bool = False):
         if dist.is_available() and dist.is_initialized() and dist.get_world_size(group) > 1:
@@ -102,6 +150,8 @@ class PeerGradBucket(FlatGradBucket):
         # parameters whose gradient is non-zero for every Gaussian on every rank (a loss term that depends on the parameters
         # alone: DNRegularization's min-scale term on `scales`): their segment is gathered from all ranks, not by `touched`
         self.dense_params = {"scales"} & set(ps)
+        # dense zero_() and per-backward flags (dnr_raster_bwd clears them): the sparse single-GPU path is not used here
+        self.sparse_ok, self.flags_valid, self._clean = False, False, False
         base = [int(x) for x in self._handle.buffer_ptrs]
         self.peer_flat = base
         self.peer_touched = [b + self._flat_bytes for b in base]

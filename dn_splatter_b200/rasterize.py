@@ -417,7 +417,18 @@ class _DnRasterize(torch.autograd.Function):
 
         v_rgb, v_depth, v_alpha = prep(v_rgb), prep(v_depth), prep(v_alpha)
         v_normal = prep(v_normal) if s.render_normals else None
-        grad_records = torch.empty(n, L.GRAD_FLOATS, **f32)
+        sink = ctx.grad_sink
+        touched = grad_records = None
+        if s.touched_bwd and not s.compact_bwd:
+            if sink is not None:
+                # the caller's buffers: a FlatGradBucket keeps the flags across backwards and grad_records always zero
+                # (DNR_FLAG_PERSISTENT_WS); parallel.PeerGradBucket's peers read its flags over NVLink
+                touched, grad_records = sink.get("touched"), sink.get("grad_records")
+            if touched is None:
+                touched, grad_records = torch.empty(n, dtype=torch.uint8, device=dev), None
+        persistent = grad_records is not None
+        if grad_records is None:
+            grad_records = torch.empty(n, L.GRAD_FLOATS, **f32)
         a = _base_args(s, n, ctx.sh_bases)
         _set_host_cam(a, ctx.host_cam)
         a.n_isects = ctx.n_isects
@@ -429,16 +440,11 @@ class _DnRasterize(torch.autograd.Function):
              v_normal=v_normal, v_alpha=v_alpha, grad_records=grad_records, stats=ctx.holder.get("stats"))
         # losses whose backward asked to be evaluated in the raster kernel's prologue (regularization_strategy.py)
         keep = _apply_deferred_losses(a, ctx.holder.pop("deferred", None))
-        touched = None
-        if s.touched_bwd and not s.compact_bwd:
-            # the caller's buffer when it wants the flags (parallel.PeerGradBucket: peers read them over NVLink)
-            touched = ctx.grad_sink.get("touched") if ctx.grad_sink is not None else None
-            if touched is None:
-                touched = torch.empty(n, dtype=torch.uint8, device=dev)
-            _set(a, touched=touched)
+        _set(a, touched=touched)
+        if persistent:
+            a.flags |= L.FLAG_PERSISTENT_WS
         L.check(_timed("raster_bwd", lib.dnr_raster_bwd, C.byref(a), st), "dnr_raster_bwd")
         del keep
-        sink = ctx.grad_sink
         if s.compact_bwd:
             a.flags |= L.FLAG_COMPACT_BWD
             a.depth_order = lib.dnr_depth_order_ptr(ctx.ws_scan.data_ptr(), n)
@@ -469,6 +475,8 @@ class _DnRasterize(torch.autograd.Function):
         S["means2d"].grad = v_m2d
         S["means2d"].absgrad = v_m2d_abs
         if sink is not None:
+            if sink.get("bucket") is not None:
+                sink["bucket"].note_backward(persistent)
             return (None,) * 11
         return (v_means, v_quats, v_scales, v_opac.view(ctx.opac_shape), v_sh_dc, v_sh_rest, None, None, None, None, None)
 

@@ -54,6 +54,10 @@ extern "C" {
 #define DNR_FLAG_HOST_CAMERA 32u /* camera passed by value in host_cam[] (no device reads, no H2D copy) */
 #define DNR_FLAG_EXACT_LISTS 16u /* parity mode: emit gsplat's full bbox intersection lists (no precise-hit cull) */
 #define DNR_FLAG_TOUCHED_BWD 128u /* project_bwd processes only Gaussians with touched[g] != 0 (needs DNR_FLAG_ACCUMULATE) */
+#define DNR_FLAG_PERSISTENT_WS 256u /* raster_bwd: touched and grad_records are the caller's persistent buffers and are not
+                                       cleared.  grad_records must be all zero on entry (the DNR_FLAG_TOUCHED_BWD project_bwd
+                                       that follows leaves it so); the flags accumulate over calls until the caller clears
+                                       them (dnr_grad_zero) */
 
 /* floats per packed per-Gaussian raster record, without / with normals */
 #define DNR_REC_FLOATS 12
@@ -129,7 +133,8 @@ typedef struct DnrArgs {
   const float* v_depth;  /* [H,W]   or NULL */
   const float* v_normal; /* [H,W,3] or NULL */
   const float* v_alpha;  /* [H,W]   or NULL */
-  float* grad_records;   /* [N, DNR_GRAD_FLOATS] zeroed by dnr_raster_bwd */
+  float* grad_records;   /* [N, DNR_GRAD_FLOATS] zeroed by dnr_raster_bwd (unless DNR_FLAG_PERSISTENT_WS); the
+                            DNR_FLAG_TOUCHED_BWD project_bwd writes zeros back to every row it consumes */
 
   /* ---- projection backward outputs ---- */
   float* v_means;       /* [N,3] */
@@ -166,7 +171,8 @@ typedef struct DnrArgs {
   const void* gt_image;  /* [H,W,3] photometric target: uint8 (DNR_LOSS_IMG_U8, scaled by 1/255) or fp32 */
   const float* v_l1;     /* [1] device scalar */
   uint8_t* touched;      /* [N] or NULL: dnr_raster_bwd sets touched[g] = 1 for every Gaussian that received a gradient
-                            (zeroed by the call); dnr_project_bwd then skips the others (DNR_FLAG_TOUCHED_BWD) */
+                            (zeroed by the call unless DNR_FLAG_PERSISTENT_WS); dnr_project_bwd then skips the others
+                            (DNR_FLAG_TOUCHED_BWD) */
   uint64_t* stats; /* [4] or NULL: += {list entries walked, entries kept by the tile filter} (fwd: [0],[1]; bwd: [2],[3]) */
 } DnrArgs;
 
@@ -276,7 +282,9 @@ int dnr_adam_step(const DnrAdamSeg* segs /* HOST array */, int32_t n_segs, doubl
  * is the sum, in rank order, of the rows of the ranks that touched the Gaussian (read straight from their memory), so
  * all replicas apply bit-identical updates.  segs[i].g must point into THIS rank's bucket (peer_flat[rank]); widths[i] =
  * floats per Gaussian of segment i.  The caller brackets the call with cross-rank barriers (all buckets final before,
- * all reads done before anyone zeroes its bucket again). */
+ * all reads done before anyone zeroes its bucket again).
+ * world == 1 is the single-GPU sparse step: peer_touched[0] (the bucket's own flags, which must cover every non-zero row
+ * of the segments not marked dense) is the mask, `mask` is unused and no barrier is needed. */
 #define DNR_PEER_MAX 8
 typedef struct DnrPeerReduce {
   int32_t world, rank;
@@ -287,6 +295,17 @@ typedef struct DnrPeerReduce {
 } DnrPeerReduce;
 int dnr_adam_step_reduce(const DnrAdamSeg* segs /* HOST array */, const int32_t* widths /* HOST array */, int32_t n_segs,
                          double beta1, double beta2, const DnrPeerReduce* peers /* HOST struct */, void* stream);
+
+/* Clears a flat gradient bucket whose `touched` flags cover every non-zero row (DNR_FLAG_PERSISTENT_WS): the rows of
+ * flagged Gaussians in each segment, every segment marked dense, and the flags themselves.  Each g starts on a 16-byte
+ * boundary and its segment is padded with zeros to a multiple of 4 floats (the padding may be written). */
+typedef struct DnrGradSeg {
+  float* g;      /* [n_gauss * width] */
+  int32_t width; /* floats per Gaussian */
+  int32_t dense; /* != 0: zero the whole segment (a gradient term that depends on the parameters alone) */
+} DnrGradSeg;
+int dnr_grad_zero(const DnrGradSeg* segs /* HOST array, at most DNR_ADAM_MAX_SEGS */, int32_t n_segs, uint8_t* touched,
+                  int32_t n_gauss, void* stream);
 
 /* ---- SuGaR-style queries (SURVEY 8f-4; Python surface: dn_splatter_b200.sugar) ----
  * Grid-hash k-NN: replaces sklearn behind dn_splatter/utils/knn.py:29-43 (knn_sk) and nerfstudio's k_nearest_sklearn
