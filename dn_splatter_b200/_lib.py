@@ -45,6 +45,7 @@ class DnrArgs(C.Structure):
         ("host_cam", _f * 32),
         ("depth_order", _p),
         ("loss_flags", C.c_uint32), ("variant", _i), ("gt_image", _p), ("v_l1", _p), ("touched", _p), ("stats", _p),
+        ("v_viewmat", _p),
     ]
 
 

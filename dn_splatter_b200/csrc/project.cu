@@ -357,9 +357,14 @@ constexpr int PB_REST_MAX = 45;    // (16 - 1) * 3 floats of higher-order SH gra
 // Parameter gradients of ONE visible Gaussian from its raster-gradient record: gsplat fully_fused_projection_bwd +
 // spherical_harmonics bwd + activation / normal chain rules.  The 3*(sh_bases-1) higher-order SH gradients go to `srow`
 // (shared memory staging, written out by the caller); the rest is returned in registers.
-template <bool NORMALS>
+// VIEWMAT: also ADDS this Gaussian's d(loss)/d(viewmat) to pv[k * PB_THREADS], k over {v_W row-major [9], v_t [3]} (the
+// thread's column of a shared-memory accumulator: keeps 12 sums out of the register budget).  With mc = W p + t,
+// Sc = W S W^T and dir = p - campos = p + W^T t:
+//   v_W += vmc p^T + 2 vSc W S + t vdir^T,   v_t += vmc + W vdir
+// (vSc is symmetric; the normals' c2w is a separate, un-optimised input and contributes nothing).
+template <bool NORMALS, bool VIEWMAT = false>
 __device__ __forceinline__ void project_bwd_gauss(const DnrArgs& a, int i, int nrest, float* srow, float vm[3], float vq[4],
-                                                  float vs[3], float& vo, float vdc[3]) {
+                                                  float vs[3], float& vo, float vdc[3], float* pv = nullptr) {
   Cam cam;
   load_cam(a, cam);
   Geo g;
@@ -443,6 +448,20 @@ __device__ __forceinline__ void project_bwd_gauss(const DnrArgs& a, int i, int n
   for (int r = 0; r < 3; ++r)
 #pragma unroll
     for (int c = 0; c < 3; ++c) vS[r][c] = cam.W[0][r] * tmp[0][c] + cam.W[1][r] * tmp[1][c] + cam.W[2][r] * tmp[2][c];
+  if constexpr (VIEWMAT) {
+    // v_W += vmc p^T + 2 (vSc W) M M^T ;  v_t += vmc
+    const float p[3] = {a.means[i * 3 + 0], a.means[i * 3 + 1], a.means[i * 3 + 2]};
+#pragma unroll
+    for (int r = 0; r < 3; ++r) {
+      float u[3];
+#pragma unroll
+      for (int j = 0; j < 3; ++j) u[j] = tmp[r][0] * g.M[0][j] + tmp[r][1] * g.M[1][j] + tmp[r][2] * g.M[2][j];
+#pragma unroll
+      for (int c = 0; c < 3; ++c)
+        pv[(r * 3 + c) * PB_THREADS] += vmc[r] * p[c] + 2.0f * (u[0] * g.M[c][0] + u[1] * g.M[c][1] + u[2] * g.M[c][2]);
+      pv[(9 + r) * PB_THREADS] += vmc[r];
+    }
+  }
   // v_M = (vS + vS^T) M
   float vM[3][3];
 #pragma unroll
@@ -545,7 +564,41 @@ __device__ __forceinline__ void project_bwd_gauss(const DnrArgs& a, int i, int n
       vm[0] += (vu[0] - ux * dp) * inorm;
       vm[1] += (vu[1] - uy * dp) * inorm;
       vm[2] += (vu[2] - uz * dp) * inorm;
+      if constexpr (VIEWMAT) {
+        // campos = -W^T t:  v_W += t vdir^T ;  v_t += W vdir
+        const float vdir[3] = {(vu[0] - ux * dp) * inorm, (vu[1] - uy * dp) * inorm, (vu[2] - uz * dp) * inorm};
+#pragma unroll
+        for (int r = 0; r < 3; ++r) {
+#pragma unroll
+          for (int c = 0; c < 3; ++c) pv[(r * 3 + c) * PB_THREADS] += cam.t[r] * vdir[c];
+          pv[(9 + r) * PB_THREADS] += cam.W[r][0] * vdir[0] + cam.W[r][1] * vdir[1] + cam.W[r][2] * vdir[2];
+        }
+      }
     }
+  }
+}
+
+// Adds the CTA's per-thread viewmat partials into v_viewmat[4,4] with 12 float atomics per CTA: s_pv[k * PB_THREADS +
+// tid] holds thread tid's sum of component k (v_W row-major [9], v_t [3]); warp shuffles, then one 12-float row per
+// warp in shared memory.  Every thread of the CTA must call it.
+__device__ __forceinline__ void cta_add_viewmat(const float* s_pv, float* v_viewmat) {
+  __shared__ float s_red[PB_THREADS / 32][12];
+  const int lane = threadIdx.x & 31, warp = threadIdx.x >> 5;
+  __syncthreads();
+#pragma unroll
+  for (int k = 0; k < 12; ++k) {
+    float v = s_pv[k * PB_THREADS + threadIdx.x];
+#pragma unroll
+    for (int off = 16; off > 0; off >>= 1) v += __shfl_xor_sync(0xffffffffu, v, off);
+    if (lane == 0) s_red[warp][k] = v;
+  }
+  __syncthreads();
+  if (threadIdx.x < 12) {
+    const int k = threadIdx.x;
+    float s = 0.f;
+#pragma unroll
+    for (int w = 0; w < PB_THREADS / 32; ++w) s += s_red[w][k];
+    atomicAdd(v_viewmat + (k < 9 ? (k / 3) * 4 + k % 3 : (k - 9) * 4 + 3), s);
   }
 }
 
@@ -554,8 +607,11 @@ __device__ __forceinline__ void project_bwd_gauss(const DnrArgs& a, int i, int n
 // COMPACT (DNR_FLAG_COMPACT_BWD, kept for A/B; the touched-flag kernel below is the default): slot s of the grid handles Gaussian depth_order[s]; the visible ones
 // come first in that order, so full CTAs do useful work and the tail CTAs leave after one load.  Rows are then
 // scattered, hence accumulate-only.
-template <bool NORMALS, bool COMPACT>
+// VIEWMAT (not with COMPACT): also adds d(loss)/d(viewmat) into a.v_viewmat, one CTA reduction at the end; a CTA that
+// leaves early at the __syncthreads_or below has no visible Gaussian and contributes zero.
+template <bool NORMALS, bool COMPACT, bool VIEWMAT = false>
 __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_kernel(const DnrArgs a) {
+  static_assert(!(COMPACT && VIEWMAT), "the compact path does not compute viewmat gradients");
   __shared__ float s_rest[PB_THREADS * PB_REST_MAX];
   __shared__ unsigned char s_vis[PB_THREADS];
   __shared__ unsigned char s_list[PB_THREADS];
@@ -585,13 +641,21 @@ __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_kernel(const DnrArg
   }
   if (acc && !__syncthreads_or(visible ? 1 : 0)) return;  // nothing to accumulate from this CTA
   float vm[3] = {0, 0, 0}, vq[4] = {0, 0, 0, 0}, vs[3] = {0, 0, 0}, vo = 0.f, vdc[3] = {0, 0, 0};
+  __shared__ float s_pv[VIEWMAT ? 12 * PB_THREADS : 1];
+  float* pv = VIEWMAT ? s_pv + threadIdx.x : nullptr;
+  if constexpr (VIEWMAT) {
+#pragma unroll
+    for (int k = 0; k < 12; ++k) pv[k * PB_THREADS] = 0.f;
+  }
   if (in_range && !visible && !acc) {
     for (int k = 0; k < 3; ++k) { a.v_means[i * 3 + k] = 0.f; a.v_scales[i * 3 + k] = 0.f; a.v_sh_dc[i * 3 + k] = 0.f; }
     for (int k = 0; k < 4; ++k) a.v_quats[i * 4 + k] = 0.f;
     a.v_opacities[i] = 0.f;
   }
-  if (visible) project_bwd_gauss<NORMALS>(a, i, nrest, srow, vm, vq, vs, vo, vdc);
-  if (acc) {
+  if (visible) project_bwd_gauss<NORMALS, VIEWMAT>(a, i, nrest, srow, vm, vq, vs, vo, vdc, pv);
+  if (!in_range) {
+    // the last CTA's lanes past n_gauss own no row (they only take part in the barriers below)
+  } else if (acc) {
     for (int k = 0; k < 3; ++k) { a.v_means[i * 3 + k] += vm[k]; a.v_scales[i * 3 + k] += vs[k]; a.v_sh_dc[i * 3 + k] += vdc[k]; }
     for (int k = 0; k < 4; ++k) a.v_quats[i * 4 + k] += vq[k];
     a.v_opacities[i] += vo;
@@ -630,6 +694,7 @@ __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_kernel(const DnrArg
       }
     }
   }
+  if constexpr (VIEWMAT) cta_add_viewmat(s_pv, a.v_viewmat);
 }
 
 // DNR_FLAG_TOUCHED_BWD: only Gaussians that received a raster gradient are processed (touched[g] != 0, written by
@@ -641,7 +706,8 @@ __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_kernel(const DnrArg
 // gradient buffers (and v_means2d / v_means2d_abs).
 constexpr int PB_SCAN = 1024;
 
-template <bool NORMALS>
+// VIEWMAT: each thread sums its Gaussians' d(loss)/d(viewmat) over the loop; one CTA reduction adds it to a.v_viewmat.
+template <bool NORMALS, bool VIEWMAT = false>
 __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_touched_kernel(const DnrArgs a) {
   __shared__ float s_rest[PB_THREADS * PB_REST_MAX];
   __shared__ int s_ids[PB_SCAN];
@@ -673,6 +739,12 @@ __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_touched_kernel(cons
   const int nrest = a.sh_bases - 1;
   const int nrow = nrest * 3;
   float* srow = s_rest + tid * PB_REST_MAX;
+  __shared__ float s_pv[VIEWMAT ? 12 * PB_THREADS : 1];
+  float* pv = VIEWMAT ? s_pv + tid : nullptr;
+  if constexpr (VIEWMAT) {
+#pragma unroll
+    for (int k = 0; k < 12; ++k) pv[k * PB_THREADS] = 0.f;
+  }
   for (int off = 0; off < n_touched; off += PB_THREADS) {
     const int slot = off + tid;
     const bool active = slot < n_touched;
@@ -680,7 +752,7 @@ __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_touched_kernel(cons
       const int i = s_ids[slot];
       float vm[3] = {0, 0, 0}, vq[4] = {0, 0, 0, 0}, vs[3] = {0, 0, 0}, vo = 0.f, vdc[3] = {0, 0, 0};
       if (a.radii[i] > 0) {
-        project_bwd_gauss<NORMALS>(a, i, nrest, srow, vm, vq, vs, vo, vdc);
+        project_bwd_gauss<NORMALS, VIEWMAT>(a, i, nrest, srow, vm, vq, vs, vo, vdc, pv);
       } else {
         for (int k = 0; k < nrow; ++k) srow[k] = 0.f;
       }
@@ -703,6 +775,9 @@ __global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_touched_kernel(cons
       }
     }
     __syncthreads();
+  }
+  if constexpr (VIEWMAT) {
+    if (n_touched > 0) cta_add_viewmat(s_pv, a.v_viewmat);
   }
 }
 
@@ -744,17 +819,27 @@ extern "C" int dnr_project_bwd(const DnrArgs* a, void* stream) {
   if (a->sh_bases > 16) return DNR_E_OPTION;
   const int block = PB_THREADS, grid = (a->n_gauss + block - 1) / block;
   cudaStream_t s = (cudaStream_t)stream;
+  const bool vmat = a->v_viewmat != nullptr;
   if (a->flags & DNR_FLAG_TOUCHED_BWD) {
     if (!a->touched) return DNR_E_NULL;
     if (!(a->flags & DNR_FLAG_ACCUMULATE)) return DNR_E_OPTION;  // scattered rows: the caller pre-zeroes and accumulates
     const int tgrid = (a->n_gauss + PB_SCAN - 1) / PB_SCAN;
-    if (normals) project_bwd_touched_kernel<true><<<tgrid, block, 0, s>>>(*a);
-    else project_bwd_touched_kernel<false><<<tgrid, block, 0, s>>>(*a);
+    if (vmat) {
+      if (normals) project_bwd_touched_kernel<true, true><<<tgrid, block, 0, s>>>(*a);
+      else project_bwd_touched_kernel<false, true><<<tgrid, block, 0, s>>>(*a);
+    } else {
+      if (normals) project_bwd_touched_kernel<true><<<tgrid, block, 0, s>>>(*a);
+      else project_bwd_touched_kernel<false><<<tgrid, block, 0, s>>>(*a);
+    }
   } else if (a->flags & DNR_FLAG_COMPACT_BWD) {
+    if (vmat) return DNR_E_OPTION;  // the compact A/B path has no viewmat gradient
     if (!a->depth_order) return DNR_E_NULL;
     if (!(a->flags & DNR_FLAG_ACCUMULATE)) return DNR_E_OPTION;  // scattered rows: the caller pre-zeroes and accumulates
     if (normals) project_bwd_kernel<true, true><<<grid, block, 0, s>>>(*a);
     else project_bwd_kernel<false, true><<<grid, block, 0, s>>>(*a);
+  } else if (vmat) {
+    if (normals) project_bwd_kernel<true, false, true><<<grid, block, 0, s>>>(*a);
+    else project_bwd_kernel<false, false, true><<<grid, block, 0, s>>>(*a);
   } else {
     if (normals) project_bwd_kernel<true, false><<<grid, block, 0, s>>>(*a);
     else project_bwd_kernel<false, false><<<grid, block, 0, s>>>(*a);

@@ -6,7 +6,8 @@ The class works standalone (nerfstudio is optional): cameras are duck-typed (cam
 nerfstudio's), parameters keep the reference's names so checkpoints stay interchangeable
 (gauss_params: means, scales, quats, features_dc, features_rest, opacities, normals).
 What is deliberately NOT here: densification (refinement_after), metrics/LPIPS, SuGaR density helpers,
-crop boxes, camera optimisation — outside the hot path (SURVEY.md §2.1 #1, §8f).
+crop boxes — outside the hot path (SURVEY.md §2.1 #1, §8f).  Camera optimisation (camera_opt.py) renders the
+training views with the optimised pose; the projection backward returns the pose gradient.
 """
 from __future__ import annotations
 
@@ -18,6 +19,7 @@ import torch
 import torch.nn.functional as F
 from torch import Tensor
 
+from .camera_opt import compose as compose_pose
 from .cameras import Cameras, is_camera
 from .losses import DepthLoss, DepthLossType, TVLoss, ssim  # noqa: F401  (ssim re-exported)
 from .rasterize import dn_rasterize, get_viewmat, raster_holder, to_device_async
@@ -101,10 +103,7 @@ try:  # nerfstudio is optional: with it the config / model classes below extend 
 except Exception:  # noqa: BLE001
     HAVE_NERFSTUDIO = False
     _ModelBase = torch.nn.Module
-
-    @dataclass
-    class CameraOptimizerConfig:  # stand-in with the one field the hot path reads (nerfstudio CameraOptimizerConfig.mode)
-        mode: Literal["off", "SO3xR3", "SE3"] = "off"
+    from .camera_opt import CameraOptimizerConfig  # stand-in for nerfstudio's (camera_opt.py)
 
     @dataclass
     class _ConfigBase:  # no inherited fields: they are spelled out below with nerfstudio 1.1.3's defaults
@@ -144,7 +143,7 @@ class DNSplatterModelConfig(_ConfigBase):
     max_gauss_ratio: float = 5.0
     stop_split_at: int = 15000
     camera_optimizer: CameraOptimizerConfig = field(default_factory=lambda: CameraOptimizerConfig(mode="off"))
-    """Config of the camera optimizer to use (reference dn_model.py:113-116); only mode == "off" is accelerated."""
+    """Config of the camera optimizer to use (reference dn_model.py:113-116): "off", "SO3xR3" or "SE3"."""
     output_depth_during_training: bool = True
     pearson_lambda: float = 0
     # ---- inherited splatfacto fields [EXT nerfstudio 1.1.3 defaults] ----
@@ -318,6 +317,8 @@ class DNSplatterModel(_ModelBase):
             rs.depth_loss_type, rs.depth_loss = None, None
         if not cfg.use_normal_loss:
             rs.normal_loss = None
+        # reference :245-247; moved to the model's device with the module.  No RNG draw (zero-initialised).
+        self.camera_optimizer = cfg.camera_optimizer.setup(num_cameras=self.num_train_data, device="cpu")
 
     # ------------------------------------------------------------------ parameter views
     means = property(lambda self: self.gauss_params["means"])
@@ -344,7 +345,10 @@ class DNSplatterModel(_ModelBase):
                                                      "opacities", "normals")}
 
     def get_param_groups(self):
-        return self.get_gaussian_param_groups()
+        """SplatfactoModel.get_param_groups [EXT]: the Gaussian groups plus "camera_opt" unless the mode is "off"."""
+        groups = self.get_gaussian_param_groups()
+        self.camera_optimizer.get_param_groups(param_groups=groups)
+        return groups
 
     # ------------------------------------------------------------------ helpers [EXT splatfacto]
     def _get_downscale_factor(self) -> int:
@@ -391,9 +395,16 @@ class DNSplatterModel(_ModelBase):
         cfg = self.config
         if self.training:
             assert camera.shape[0] == 1, "Only one camera at a time"
-        if cfg.camera_optimizer_mode != "off":
-            raise NotImplementedError("camera optimisation is outside the accelerated hot path")
-        c2w_opt = camera.camera_to_worlds
+        # camera optimisation (reference :420-425): training views with metadata["cam_idx"] render with the optimised pose;
+        # evaluation, mode "off" and views without an index use the pose as given
+        cam_idx = None
+        if self.training and cfg.camera_optimizer_mode != "off":
+            meta = getattr(camera, "metadata", None)
+            if meta and "cam_idx" in meta:
+                cam_idx = int(meta["cam_idx"])
+                if not 0 <= cam_idx < self.num_train_data:
+                    raise ValueError(f"camera optimisation: cam_idx {cam_idx} is not one of the model's "
+                                     f"{self.num_train_data} training cameras (num_train_data)")
         if cfg.use_binary_opacities and self.step > cfg.warmup_length:  # reference :427-437
             skip = cfg.reset_alpha_every * cfg.refine_every
             if self.step % skip != 0 and self.step % skip not in range(1, 201):
@@ -410,7 +421,7 @@ class DNSplatterModel(_ModelBase):
         camera.rescale_output_resolution(1 / scale_fac)
         dev = self.device
         # Per-camera constants are cached on the camera object as HOST tensors and handed to the kernels by value:
-        # the step issues no H2D copy and no device op for the camera (camera optimisation is off on this path).
+        # the step issues no H2D copy and no device op for the camera (unless its pose is optimised, below).
         cache = camera.__dict__.setdefault("_dnr_cache", {})
         pose = camera.camera_to_worlds
         key = (scale_fac, pose.data_ptr(), pose._version)  # an in-place pose update invalidates the entry
@@ -420,10 +431,20 @@ class DNSplatterModel(_ModelBase):
             cache[key] = (camera.get_intrinsics_matrices()[0].float().cpu(), int(camera.width.flatten()[0]),
                           int(camera.height.flatten()[0]), c2w_host, get_viewmat(c2w_host))
         K, W, H, c2w_fixed, viewmat = cache[key]
+        if cam_idx is not None:  # the pose gradient needs a device viewmat: device copies of K and the un-optimised c2w
+            dkey = (key, str(dev))
+            if dkey not in cache:
+                cache[dkey] = (to_device_async(K, dev), to_device_async(c2w_fixed, dev))
+            K, c2w_fixed = cache[dkey]
         fixed_capacity = 0
         gc = self.__dict__.get("_graph_cam")
         if gc is not None:  # CUDA-graph mode: camera in static device buffers (refreshed before each replay), fixed capacity
             K, c2w_fixed, viewmat, fixed_capacity = gc.K, gc.c2w, gc.viewmat, gc.capacity
+        if cam_idx is not None:
+            # c2w @ exp(pose_adjustment[cam_idx]) on the device; in graph mode the row index is a device tensor too.  The
+            # normals keep the un-optimised, detached c2w (reference :550-560).
+            rows = gc.cam_idx if gc is not None else slice(cam_idx, cam_idx + 1)
+            viewmat = get_viewmat(compose_pose(c2w_fixed.reshape(1, 3, 4), self.camera_optimizer(rows)))
         self.last_size = (H, W)
         camera.rescale_output_resolution(scale_fac)
         sh_degree_to_use = min(self.step // cfg.sh_degree_interval, cfg.sh_degree)

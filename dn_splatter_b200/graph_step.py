@@ -28,12 +28,16 @@ from .rasterize import GROWTH, CountWatch, get_viewmat, grow, suggested_capacity
 
 class StaticCamera:
     """What get_outputs renders with while installed as the model's `_graph_cam`: the static device camera block
-    [viewmat 16 | K 9 | c2w 12], read through `viewmat` / `K` / `c2w`, and the graph's fixed intersection `capacity`."""
+    [viewmat 16 | K 9 | c2w 12], read through `viewmat` / `K` / `c2w`, and the graph's fixed intersection `capacity`.
+    With `num_cameras` (camera optimisation) also the view's metadata["cam_idx"] as a device int64 [1], `cam_idx`: the
+    graph selects the view's pose_adjustment row with it."""
 
-    def __init__(self, size: Tuple[int, int], device, capacity: int):
+    def __init__(self, size: Tuple[int, int], device, capacity: int, num_cameras: Optional[int] = None):
         self.size, self.capacity = size, int(capacity)
         self.data = torch.zeros(37, device=device)
         self.viewmat, self.K, self.c2w = self.data[:16].view(4, 4), self.data[16:25].view(3, 3), self.data[25:].view(3, 4)
+        self.num_cameras = num_cameras
+        self.cam_idx = torch.zeros(1, dtype=torch.int64, device=device) if num_cameras is not None else None
 
     def load(self, camera) -> None:
         """Refreshes the block from a camera: ONE 148-byte async H2D copy from a per-camera pinned tensor
@@ -45,6 +49,17 @@ class StaticCamera:
             pinned = torch.cat([get_viewmat(c2w).reshape(-1), camera.get_intrinsics_matrices()[0].float().cpu().reshape(-1),
                                 c2w.reshape(-1)]).contiguous().pin_memory()
             camera.__dict__["_dnr_graph_cam"] = pinned
+        if self.cam_idx is not None:
+            metadata = getattr(camera, "metadata", None)
+            if not metadata or "cam_idx" not in metadata:
+                raise ValueError("camera optimisation in a captured step needs metadata['cam_idx'] on every camera")
+            if not 0 <= int(metadata["cam_idx"]) < self.num_cameras:
+                raise ValueError(f"cam_idx {int(metadata['cam_idx'])} is not one of the {self.num_cameras} training cameras")
+            idx = camera.__dict__.get("_dnr_graph_idx")
+            if idx is None or int(idx[0]) != int(metadata["cam_idx"]):
+                idx = torch.tensor([int(metadata["cam_idx"])], dtype=torch.int64).pin_memory()
+                camera.__dict__["_dnr_graph_idx"] = idx
+            self.cam_idx.copy_(idx, non_blocking=True)
         self.data.copy_(pinned, non_blocking=True)
 
 
@@ -87,7 +102,13 @@ class GraphedTrainStep:
                                           cfg.list_shift)
         if capacity <= 0:
             raise ValueError("no intersection statistics yet: run a few sync_free views first or pass capacity=")
-        self.cam = StaticCamera((W, H), dev, capacity)
+        cam_opt = model.config.camera_optimizer_mode != "off"
+        self.cam = StaticCamera((W, H), dev, capacity, num_cameras=model.num_train_data if cam_opt else None)
+        if cam_opt:
+            # replays accumulate the pose gradient into a buffer whose address the graph baked in
+            pa = model.camera_optimizer.pose_adjustment
+            if pa.grad is None:
+                pa.grad = torch.zeros_like(pa)
         self.batches: List[Dict[str, Tensor]] = [
             {k: torch.empty_like(v, device=dev) for k, v in example_batch.items()} for _ in range(n_slots)]
         self.losses = [torch.zeros((), device=dev) for _ in range(n_slots)]
@@ -128,7 +149,12 @@ class GraphedTrainStep:
             if name in model.__dict__:
                 model.__dict__[name] = None
         gc.collect()
+        # the warm-up runs add real pose gradients: keep the accumulation window's gradient as it was
+        pa = model.camera_optimizer.pose_adjustment if self.cam.cam_idx is not None else None
+        saved = pa.grad.clone() if pa is not None else None
         self.graphs, self._count_dev = capture_slots(self._eager, self._n_slots, self._warmup, self.device)
+        if pa is not None:
+            pa.grad.copy_(saved)
 
     def _eager(self, slot: int) -> Tensor:
         m = self.model

@@ -258,6 +258,7 @@ class _DnRasterize(torch.autograd.Function):
         s = settings
         ctx.set_materialize_grads(False)  # unused output gradients arrive as None instead of freshly filled zero tensors
         dev = _require_cuda(means, quats, scales, opacities, sh_dc, sh_rest)
+        ctx.viewmat_meta = (viewmat.shape, viewmat.device)
         # camera on the host (CPU tensors) -> passed by value, no device traffic; on the device -> read by the kernels
         host_cam = None
         if viewmat.device.type == "cpu":
@@ -468,17 +469,24 @@ class _DnRasterize(torch.autograd.Function):
             v_sh_rest = alloc(sh_rest)
         v_m2d = (torch.zeros if touched is not None else torch.empty)(n, 2, **f32)
         v_m2d_abs = (torch.zeros if touched is not None else torch.empty)(n, 2, **f32)
+        # camera optimisation: d(loss)/d(viewmat) only when the viewmat asks for it (otherwise the launch is unchanged)
+        v_viewmat = torch.zeros(4, 4, **f32) if ctx.needs_input_grad[6] else None
         _set(a, v_means=v_means, v_quats=v_quats, v_scales=v_scales, v_opacities=v_opac, v_sh_dc=v_sh_dc,
-             v_sh_rest=v_sh_rest if ctx.sh_bases > 1 else None, v_means2d=v_m2d, v_means2d_abs=v_m2d_abs)
+             v_sh_rest=v_sh_rest if ctx.sh_bases > 1 else None, v_means2d=v_m2d, v_means2d_abs=v_m2d_abs,
+             v_viewmat=v_viewmat)
         L.check(_timed("project_bwd", lib.dnr_project_bwd, C.byref(a), st), "dnr_project_bwd")
         # what nerfstudio's after_train reads: self.xys.grad / self.xys.absgrad (dn_model.py:517-519)
         S["means2d"].grad = v_m2d
         S["means2d"].absgrad = v_m2d_abs
+        if v_viewmat is not None:
+            shape, vdev = ctx.viewmat_meta
+            v_viewmat = v_viewmat.to(vdev).view(shape)
         if sink is not None:
             if sink.get("bucket") is not None:
                 sink["bucket"].note_backward(persistent)
-            return (None,) * 11
-        return (v_means, v_quats, v_scales, v_opac.view(ctx.opac_shape), v_sh_dc, v_sh_rest, None, None, None, None, None)
+            return (None,) * 6 + (v_viewmat,) + (None,) * 4
+        return (v_means, v_quats, v_scales, v_opac.view(ctx.opac_shape), v_sh_dc, v_sh_rest, v_viewmat, None, None, None,
+                None)
 
 
 def _apply_deferred_losses(a: L.DnrArgs, deferred: Optional[dict]):
@@ -584,7 +592,7 @@ def get_viewmat(c2w: Tensor) -> Tensor:
     Rinv = torch.cat([c2w[:, :1], -c2w[:, 1:3]], dim=1).T  # (R * diag(1,-1,-1))^T
     t = -(Rinv @ c2w[:, 3:4])
     bottom = torch.zeros(1, 4, dtype=c2w.dtype, device=c2w.device)
-    bottom[0, 3] = 1.0
+    bottom[:, 3:].fill_(1.0)  # a fill kernel: `bottom[0, 3] = 1.0` copies a host scalar (not capturable)
     return torch.cat([torch.cat([Rinv, t], dim=1), bottom], dim=0)
 
 

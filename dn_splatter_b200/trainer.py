@@ -1,7 +1,8 @@
 """A minimal training loop standing in for nerfstudio's Trainer [EXT] around the hot path: per-group Adam with the
 reference's learning rates (dn_config.py:29-68), the callback order of SURVEY §3.1 (step_cb -> forward -> losses ->
 backward -> [all-reduce] -> optimizer step -> after_train -> refinement every `refine_every`), per-camera sharding
-over ranks.  Eager launches (the Gaussian count changes at refinements; capture a GraphedTrainStep between them if
+over ranks.  With camera optimisation on, the "camera_opt" group has its own torch.optim.Adam, stepped with nerfstudio's
+gradient accumulation (TRAINER_DEFAULTS: every 100 steps).  Eager launches (the Gaussian count changes at refinements; capture a GraphedTrainStep between them if
 wanted)."""
 from __future__ import annotations
 
@@ -10,12 +11,13 @@ from typing import Callable, Dict, Optional
 import torch
 
 from .densify import build_optimizers, exponential_lr
-from .dn_config import MAX_NUM_ITERATIONS, optimizer_groups
+from .dn_config import MAX_NUM_ITERATIONS, TRAINER_DEFAULTS, optimizer_groups
 
 
 class Trainer:
     def __init__(self, model, next_train: Callable[[int], tuple], max_steps: int = MAX_NUM_ITERATIONS,
-                 world_size: int = 1, seed: int = 0, fused_adam: bool = False, peer_reduce: bool = False):
+                 world_size: int = 1, seed: int = 0, fused_adam: bool = False, peer_reduce: bool = False,
+                 camera_opt_accum: Optional[int] = None):
         self.model, self.next_train, self.max_steps = model, next_train, max_steps
         self.groups = optimizer_groups(max_steps)
         self.fused = None
@@ -32,6 +34,18 @@ class Trainer:
         if self.peer_reduce and self.fused is None:
             raise ValueError("peer_reduce needs fused_adam=True (the reduction is part of dnr_adam_step_reduce)")
         self.bucket = model.enable_flat_grads(peer=self.peer_reduce)
+        # camera poses: not part of FusedAdam (which steps every group every step).  nerfstudio's Trainer zeroes a group
+        # with gradient_accumulation_steps = k at step % k == 0 and steps it at step % k == k - 1 [EXT]
+        self.camera_opt: Optional[torch.optim.Optimizer] = None
+        cam_params = model.get_param_groups().get("camera_opt")
+        if cam_params:
+            g = self.groups["camera_opt"]
+            self.camera_opt = torch.optim.Adam(cam_params, lr=g["lr"], eps=g["eps"])
+            for p in cam_params:  # every rank joins the all-reduce, also one whose views had no cam_idx
+                if p.grad is None:
+                    p.grad = torch.zeros_like(p)
+        self.camera_opt_accum = int(camera_opt_accum if camera_opt_accum is not None
+                                    else TRAINER_DEFAULTS["gradient_accumulation_steps"]["camera_opt"])
         self.world_size = world_size
         self.generator = torch.Generator().manual_seed(seed)  # identical on every rank: identical split samples
         self.step = 0
@@ -43,6 +57,8 @@ class Trainer:
         camera, batch = self.next_train(step)
         self.bucket = m._bucket or m.enable_flat_grads()
         self.bucket.zero_()
+        if self.camera_opt is not None and step % self.camera_opt_accum == 0:
+            self.camera_opt.zero_grad(set_to_none=False)  # keeps the gradient's address (a captured step accumulates there)
         outputs = m.get_outputs(camera)
         loss_dict = m.get_loss_dict(outputs, batch)
         loss = loss_dict["main_loss"] + loss_dict["scale_reg"]
@@ -61,6 +77,8 @@ class Trainer:
             self.fused.step_reduce(self.bucket)
         elif self.fused is not None:
             self.fused.step()
+        if self.camera_opt is not None:
+            self._camera_opt_step(step)
         m.after_train(step)
         info: Optional[Dict[str, int]] = None
         if step > 0 and step % m.config.refine_every == 0:
@@ -73,3 +91,18 @@ class Trainer:
             info = m.refinement_after(self.optimizers, step, generator=self.generator)
         self.step += 1
         return {"loss": loss.detach(), "refine": info}
+
+    def _camera_opt_step(self, step: int) -> None:
+        g = self.groups["camera_opt"]
+        for pg in self.camera_opt.param_groups:  # the scheduler advances every step
+            pg["lr"] = exponential_lr(g["lr"], g["lr_final"], step, g["max_steps"])
+        if step % self.camera_opt_accum != self.camera_opt_accum - 1:
+            return
+        if self.world_size > 1:  # every rank renders other cameras: sum the pose gradient once per accumulation window
+            import torch.distributed as dist
+
+            for pg in self.camera_opt.param_groups:
+                for p in pg["params"]:
+                    if p.grad is not None:
+                        dist.all_reduce(p.grad, op=dist.ReduceOp.SUM)
+        self.camera_opt.step()

@@ -174,6 +174,9 @@ typedef struct DnrArgs {
                             (zeroed by the call unless DNR_FLAG_PERSISTENT_WS); dnr_project_bwd then skips the others
                             (DNR_FLAG_TOUCHED_BWD) */
   uint64_t* stats; /* [4] or NULL: += {list entries walked, entries kept by the tile filter} (fwd: [0],[1]; bwd: [2],[3]) */
+  float* v_viewmat; /* [4,4] or NULL: dnr_project_bwd ADDS d(loss)/d(viewmat) (camera optimisation; the caller zeroes it
+                       first; row 3 is left alone).  Works with DNR_FLAG_HOST_CAMERA too; not with DNR_FLAG_COMPACT_BWD
+                       (DNR_E_OPTION).  The normals' c2w is treated as a separate constant. */
 } DnrArgs;
 
 /* loss_flags */

@@ -7,6 +7,8 @@ Rows (one JSON line each):
   ssim        FusedSSIM fwd+bwd  vs  dn_model.ssim (torch convs + autograd) at 1920x1080x3
   adam        FusedAdam (1 launch) vs  7 x torch.optim.Adam (default foreach) and fused=True, N Gaussians, SH degree 3
   project_bwd default vs DNR_FLAG_COMPACT_BWD on the bench scene (stage events)
+  camera_opt  project_bwd with vs without the view-matrix gradient (stage events), and the captured 1080p training step
+              (GraphedTrainStep + FusedAdam) with camera optimisation off vs SO3xR3
 Each row also checks agreement with the reference path (max abs / rel error), so a faster-but-wrong kernel is visible.
 """
 import argparse
@@ -128,6 +130,78 @@ def bench_project_bwd():
     emit({"row": "project_bwd", "default_ms": res[False], "compact_ms": res[True], "grad_rel_err": rel})
 
 
+def bench_camera_opt():
+    import dn_splatter_b200.rasterize as R
+    from dn_splatter_b200 import dn_rasterize, get_viewmat
+    from dn_splatter_b200.cameras import Cameras
+    from dn_splatter_b200.dn_model import CameraOptimizerConfig, DNSplatterModelConfig
+    from dn_splatter_b200.graph_step import GraphedTrainStep
+    from dn_splatter_b200.losses import DepthLossType
+    from dn_splatter_b200.optim import FusedAdam
+    from dn_splatter_b200.synthetic import BACKGROUND, make_scene, ring_cameras
+
+    W, H, n_views = 1920, 1080, 200
+    ring = ring_cameras(n_views, W, H)
+    row = {"row": "camera_opt", "n_gauss": args.n, "resolution": f"{W}x{H}"}
+    # project_bwd alone: the same view, with and without a viewmat that requires grad
+    cam = ring[3]
+    K = torch.tensor([[cam["fx"], 0, cam["cx"]], [0, cam["fy"], cam["cy"]], [0, 0, 1]], dtype=torch.float32, device="cuda")
+    c2w = cam["c2w"].cuda()
+    grads = {}
+    for pose_grad in (False, True):
+        p = {k: v.cuda().requires_grad_(True) for k, v in make_scene(args.n, seed=0).items()}
+        vm = get_viewmat(c2w).detach().requires_grad_(pose_grad)
+        out = dn_rasterize(p["means"], p["quats"], p["scales"], p["opacities"], p["features_dc"], p["features_rest"], vm, K, W,
+                           H, background=BACKGROUND, c2w=c2w)
+        loss = (out.rgb.sum() + out.depth.sum() * 0.1 + out.normal.sum()) * 1e-3
+        inputs = list(p.values()) + ([vm] if pose_grad else [])
+        R.STAGE_EVENTS = []
+        for _ in range(args.reps):
+            gr = torch.autograd.grad(loss, inputs, retain_graph=True)
+        torch.cuda.synchronize()
+        t = sorted(a.elapsed_time(b) for name, a, b in R.STAGE_EVENTS if name == "project_bwd")
+        R.STAGE_EVENTS = None
+        row["project_bwd_ms_pose_grad" if pose_grad else "project_bwd_ms"] = t[len(t) // 2]
+        grads[pose_grad] = gr[:6]
+    row["param_grad_rel_err"] = max(float((x - y).norm() / (x.norm() + 1e-30)) for x, y in zip(grads[False], grads[True]))
+    # the captured training step (bench.py's loss configuration) over the camera ring, Adam included
+    g = torch.Generator().manual_seed(1)
+    batch = {"image": (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8).cuda(),
+             "mono_depth": (2 + 6 * torch.rand(H, W, 1, generator=g)).cuda(),
+             "normal": (torch.rand(H, W, 3, generator=g) * 255).to(torch.uint8).cuda()}
+    for mode in ("off", "SO3xR3"):
+        cfg = DNSplatterModelConfig(random_init=True, num_random=16, use_depth_loss=True, depth_lambda=0.2,
+                                    depth_loss_type=DepthLossType.EdgeAwareLogL1, ssim_lambda=0.2, background_color="black",
+                                    sync_free=True, camera_optimizer=CameraOptimizerConfig(mode=mode))
+        m = cfg.setup(device="cuda", num_train_data=n_views)
+        m.load_gaussians(make_scene(args.n, seed=0))
+        m.step = 30000
+        m.train()
+        cams = [Cameras(c["c2w"][None], c["fx"], c["fy"], c["cx"], c["cy"], W, H, metadata={"cam_idx": i})
+                for i, c in enumerate(ring)]
+        stream = torch.cuda.Stream()
+        with torch.cuda.stream(stream):
+            bucket = m.enable_flat_grads()
+            opt = FusedAdam.for_model(m)
+            for i in range(0, n_views, 25):  # sync-free capacity statistics for the capture
+                bucket.zero_()
+                ld = m.get_loss_dict(m.get_outputs(cams[i]), dict(batch))
+                (ld["main_loss"] + ld["scale_reg"]).backward()
+            del ld
+            step = GraphedTrainStep(m, bucket, cams[0], batch, n_slots=1)
+
+            def one(s=[0]):
+                s[0] += 1
+                step(cams[(37 * s[0]) % n_views], 0)
+                opt.step()
+
+            row[f"step_ms_{mode}"] = timed(one, args.reps)
+            step.check_capacity(wait=True)
+        del step, m, bucket, opt
+        torch.cuda.empty_cache()
+    emit(row)
+
+
 def bench_knn():
     import time
 
@@ -181,7 +255,8 @@ def bench_render_service():
     emit(row)
 
 
-for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("project_bwd", bench_project_bwd), ("knn", bench_knn),
+for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("project_bwd", bench_project_bwd),
+                 ("camera_opt", bench_camera_opt), ("knn", bench_knn),
                  ("render_service", bench_render_service)):
     if args.only and name not in args.only.split(","):
         continue
