@@ -1,5 +1,7 @@
 """dn_splatter_b200 — H100-native (sm_90a) depth+normal Gaussian rasterizer behind the dn-splatter
 plugin surface.  The arithmetic lives in libdnr_b200.so (C ABI: include/dnr.h); see DESIGN.md."""
 from .rasterize import RasterOutput, RasterSettings, dn_rasterize, get_viewmat  # noqa: F401
+from .mesh import (TSDFVolume, TriangleMesh, export_marching_cubes_mesh, export_tsdf_mesh, filter_small_clusters,  # noqa: F401
+                   marching_cubes, write_ply)
 
 __version__ = "0.1.0"

@@ -78,6 +78,19 @@ class DnrKnnGrid(C.Structure):
     _fields_ = [("lo", _f * 3), ("cell", _f), ("inv_cell", _f), ("dims", C.c_int32 * 3)]
 
 
+class DnrTsdfGrid(C.Structure):
+    """Mirror of struct DnrTsdfGrid (include/dnr.h)."""
+
+    _fields_ = [("origin", _f * 3), ("voxel", _f), ("sdf_trunc", _f), ("dims", C.c_int32 * 3), ("voxels", _p)]
+
+
+class DnrMcField(C.Structure):
+    """Mirror of struct DnrMcField (include/dnr.h)."""
+
+    _fields_ = [("values", _p), ("valid", _p), ("tsdf", _p), ("dims", C.c_int32 * 3), ("iso", _f), ("origin", _f * 3),
+                ("spacing", _f)]
+
+
 POINTER_FIELDS = {n for n, t in DnrArgs._fields_ if t is _p}
 
 _lib: Optional[C.CDLL] = None
@@ -91,6 +104,7 @@ KERNELS_PER_CALL = {
     "dnr_ssim_fwd": (1, 0), "dnr_ssim_bwd": (1, 0), "dnr_ssim_fwd_ex": (1, 0), "dnr_ssim_bwd_ex": (1, 0), "dnr_photometric_fwd": (2, 0), "dnr_photometric_bwd": (1, 0), "dnr_adam_step": (1, 0), "dnr_adam_step_reduce": (2, 0),
     "dnr_grad_zero": (1, 0),
     "dnr_knn_build": (2, 1), "dnr_knn_query": (1, 0), "dnr_density": (1, 0), "dnr_ray_densities": (1, 0),
+    "dnr_tsdf_integrate": (1, 0), "dnr_mc_count": (1, 6), "dnr_mc_emit": (2, 0),
 }
 LAUNCHES = {"handwritten": 0, "cub": 0}
 DEBUG_CAPTURE = os.environ.get("DNR_DEBUG_CAPTURE") == "1"
@@ -203,6 +217,18 @@ def load():
     lib.dnr_ray_densities.restype = C.c_int
     lib.dnr_ray_densities.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p,
                                       C.c_void_p, C.c_int32, C.c_int32, C.c_float, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_tsdf_integrate.restype = C.c_int
+    lib.dnr_tsdf_integrate.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_void_p,
+                                       C.c_float, C.c_void_p]
+    lib.dnr_mc_count_workspace_bytes.restype = C.c_int64
+    lib.dnr_mc_count_workspace_bytes.argtypes = [C.c_void_p]
+    lib.dnr_mc_count.restype = C.c_int
+    lib.dnr_mc_count.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.dnr_mc_emit_workspace_bytes.restype = C.c_int64
+    lib.dnr_mc_emit_workspace_bytes.argtypes = [C.c_void_p]
+    lib.dnr_mc_emit.restype = C.c_int
+    lib.dnr_mc_emit.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                C.c_void_p]
     lib.dnr_ssim_bwd.restype = C.c_int
     lib.dnr_ssim_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
@@ -221,7 +247,8 @@ EXPORTS = (
     "dnr_bin_sort_workspace_bytes", "dnr_bin_sort", "dnr_depth_order_ptr", "dnr_raster_fwd", "dnr_finalize_fwd", "dnr_normal_from_depth",
     "dnr_raster_bwd", "dnr_project_bwd", "dnr_loss_fwd", "dnr_loss_bwd", "dnr_scale_loss_fwd", "dnr_scale_loss_bwd",
     "dnr_l1_fwd", "dnr_l1_bwd", "dnr_u8_to_f32", "dnr_ssim_fwd", "dnr_ssim_bwd", "dnr_ssim_fwd_ex", "dnr_ssim_bwd_ex", "dnr_photometric_fwd", "dnr_photometric_bwd", "dnr_adam_step", "dnr_adam_step_reduce", "dnr_grad_zero", "dnr_knn_workspace_bytes", "dnr_knn_build", "dnr_knn_query",
-    "dnr_density", "dnr_ray_densities",
+    "dnr_density", "dnr_ray_densities", "dnr_tsdf_integrate", "dnr_mc_count_workspace_bytes", "dnr_mc_count",
+    "dnr_mc_emit_workspace_bytes", "dnr_mc_emit",
 )
 
 

@@ -340,6 +340,45 @@ int dnr_ray_densities(const float* points, int64_t n_points, const int64_t* nbr_
                       int32_t n_gauss, int32_t n_range, float range_size, float* out_dens, float* out_t, float* out_dirs,
                       void* stream);
 
+/* ---- Mesh export (Python surface: dn_splatter_b200.mesh) ----
+ * Dense TSDF volume: voxel (i, j, k) is voxels[(i * dims[1] + j) * dims[2] + k] (64-bit index), 16 bytes
+ * {float tsdf, float weight, half r, half g, half b, half pad}; colour is the weighted mean of the reference's uint8
+ * colours (0..255).  Voxel centres are origin + (index + 0.5) * voxel.  All zero is an empty volume. */
+typedef struct DnrTsdfGrid {
+  float origin[3];
+  float voxel;     /* voxel edge */
+  float sdf_trunc; /* truncation distance */
+  int32_t dims[3]; /* voxels per axis, each <= 65535 */
+  void* voxels;
+} DnrTsdfGrid;
+/* Fuses one view, Open3D legacy ScalableTSDFVolume.integrate semantics (DESIGN.md §2) [EXT]: depth [H,W] f32,
+ * rgb [H,W,3] f32 in [0,1], mask [H,W] uint8 or NULL (0 = no depth), depth <= 0 or > depth_trunc is no depth.
+ * cam_host: 16 HOST floats {fx, fy, cx, cy, world->camera [3,4] row-major (OpenCV)}.  Only updated voxels are written. */
+int dnr_tsdf_integrate(const DnrTsdfGrid* grid, const float* depth, const float* rgb, const uint8_t* mask, int32_t width,
+                       int32_t height, const float* cam_host, float depth_trunc, void* stream);
+
+/* Marching cubes over samples (i, j, k) at origin + (i, j, k) * spacing, index (i * dims[1] + j) * dims[2] + k.  Exactly
+ * one of values / tsdf is set.  "Inside" is value < iso; a cube with an invalid corner emits nothing.  Vertices are welded
+ * (one per crossed grid edge), ordered by (sample index, edge axis); faces by cube index, then table order
+ * (csrc/mc_tables.cuh), counter-clockwise seen from the value > iso side. */
+typedef struct DnrMcField {
+  const float* values;  /* [X,Y,Z] scalar field, or NULL */
+  const uint8_t* valid; /* [X,Y,Z] or NULL (all valid); with values only */
+  const void* tsdf;     /* [X,Y,Z] DnrTsdfGrid voxels, or NULL: value = tsdf, valid where weight > 0, with colour */
+  int32_t dims[3];      /* samples per axis, each <= 65535 */
+  float iso;
+  float origin[3];
+  float spacing;
+} DnrMcField;
+/* Phase 1: counts_host[3] = {active cubes, triangles, vertices}; synchronises the stream (the one host read). */
+int64_t dnr_mc_count_workspace_bytes(const DnrMcField* field);
+int dnr_mc_count(const DnrMcField* field, void* ws, int64_t ws_bytes, int64_t* counts_host, void* stream);
+/* Phase 2, with the count workspace as phase 1 left it: vertices [V,3], faces [F,3] int32, colors [V,3] in [0,1] (tsdf
+ * only; may be NULL).  DNR_E_OVERFLOW past 2^31-1 vertices or faces. */
+int64_t dnr_mc_emit_workspace_bytes(const int64_t* counts_host);
+int dnr_mc_emit(const DnrMcField* field, const void* count_ws, const int64_t* counts_host, void* ws, int64_t ws_bytes,
+                float* vertices, int32_t* faces, float* colors, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

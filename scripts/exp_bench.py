@@ -9,6 +9,8 @@ Rows (one JSON line each):
   project_bwd default vs DNR_FLAG_COMPACT_BWD on the bench scene (stage events)
   camera_opt  project_bwd with vs without the view-matrix gradient (stage events), and the captured 1080p training step
               (GraphedTrainStep + FusedAdam) with camera optimisation off vs SO3xR3
+  mesh        TSDF fusion of 200 ring views at 1920x1080 into a 512^3 grid over the scene cube (render + integrate, and
+              integrate alone, from CUDA events), marching cubes of that volume, export_marching_cubes_mesh at 256^3
 Each row also checks agreement with the reference path (max abs / rel error), so a faster-but-wrong kernel is visible.
 """
 import argparse
@@ -255,9 +257,76 @@ def bench_render_service():
     emit(row)
 
 
+def bench_mesh():
+    """mesh.py on the bench scene.  Integrate's algorithmic bytes: a 16 B read + 16 B write per updated voxel plus its
+    4 B depth and 12 B rgb gathers (the depth reads of in-frustum voxels that are not updated are not counted)."""
+    import subprocess
+    import tempfile
+    import time
+
+    from dn_splatter_b200.cameras import Cameras
+    from dn_splatter_b200.dn_model import DNSplatterModelConfig
+    from dn_splatter_b200.mesh import TSDFVolume, export_marching_cubes_mesh
+    from dn_splatter_b200.render_service import ViewRenderer
+    from dn_splatter_b200.synthetic import make_scene, ring_cameras
+
+    W, H, n_views, res = 1920, 1080, 200, 512
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip().splitlines()[0]
+    m = DNSplatterModelConfig(random_init=True, num_random=16, background_color="black", sync_free=True).setup(device="cuda")
+    m.load_gaussians(make_scene(args.n, seed=0))
+    m.step = 30000
+    cams = [Cameras(c["c2w"][None], c["fx"], c["fy"], c["cx"], c["cy"], W, H) for c in ring_cameras(n_views, W, H)]
+    bounds, voxel = ((-5.0, -5.0, -5.0), (5.0, 5.0, 5.0)), 10.0 / res  # make_scene's means fill the cube [-5, 5]^3
+    row = {"row": "mesh", "card": card, "n_gauss": args.n, "views": n_views, "resolution": f"{W}x{H}"}
+    r = ViewRenderer(m, keys=("rgb", "depth"), to_host=False)
+    vol = TSDFVolume(bounds, voxel_size=voxel, sdf_trunc=3 * voxel)
+    row["grid"] = "x".join(map(str, vol.dims))
+    for idx, maps in r.render(cams[:8]):  # warm-up: captures the forward graphs
+        vol.integrate(maps["depth"], maps["rgb"], cams[idx])
+    maps = next(iter(r.render(cams[:1])))[1]
+    depth, rgb = maps["depth"].clone(), maps["rgb"].clone()
+    vol.voxels.zero_()
+    vol.integrate(depth, rgb, cams[0])
+    updated = int((vol.voxels[:, 1] > 0).sum())
+    t_int = timed(lambda: vol.integrate(depth, rgb, cams[0]), args.reps)
+    row["integrate_ms"] = t_int
+    row["integrate_updated_voxels"] = updated
+    row["integrate_gb_s"] = updated * (32 + 16) / (t_int * 1e-3) / 1e9
+    row["integrate_frac_of_3.35TB_s"] = row["integrate_gb_s"] / 3350.0
+    vol.voxels.zero_()
+    e0, e1 = torch.cuda.Event(enable_timing=True), torch.cuda.Event(enable_timing=True)
+    torch.cuda.synchronize()
+    e0.record()
+    for idx, maps in r.render(cams):
+        vol.integrate(maps["depth"], maps["rgb"], cams[idx])
+    e1.record()
+    torch.cuda.synchronize()
+    row["render_integrate_ms_per_view"] = e0.elapsed_time(e1) / n_views
+    mesh = vol.extract_mesh()
+    torch.cuda.synchronize()
+    t0 = time.perf_counter()
+    for _ in range(3):
+        mesh = vol.extract_mesh()
+    torch.cuda.synchronize()
+    row["marching_cubes_ms"] = (time.perf_counter() - t0) / 3 * 1e3
+    row["triangles"], row["vertices"] = int(mesh.faces.shape[0]), int(mesh.vertices.shape[0])
+    del vol, mesh
+    torch.cuda.empty_cache()
+    with tempfile.TemporaryDirectory() as tmp:
+        export_marching_cubes_mesh(m, cams, tmp, resolution=64)  # warm-up
+        torch.cuda.synchronize()
+        t0 = time.perf_counter()
+        mc = export_marching_cubes_mesh(m, cams, tmp, resolution=256)
+        torch.cuda.synchronize()
+        row["export_marching_cubes_256_s"] = time.perf_counter() - t0
+        row["export_marching_cubes_256_triangles"] = int(mc.faces.shape[0])
+    emit(row)
+
+
 for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("project_bwd", bench_project_bwd),
                  ("camera_opt", bench_camera_opt), ("knn", bench_knn),
-                 ("render_service", bench_render_service)):
+                 ("render_service", bench_render_service), ("mesh", bench_mesh)):
     if args.only and name not in args.only.split(","):
         continue
     try:
