@@ -260,7 +260,17 @@ def test_graphed_train_step_overflow_is_loud_and_recoverable():
         _graph_step_body(n_gauss=12000, capacity=4096)
 
 
-def _graph_step_body(n_gauss=4000, capacity=None):
+@needs_cuda
+@pytest.mark.parametrize("overflow", [False, True], ids=["fits", "overflow_recapture"])
+def test_cuda_graph_step_with_ssim_matches_eager_step(overflow):
+    """The captured step bench.py times: ssim_lambda = 0.2, so the photometric term is FusedPhotometric inside the
+    graph.  Replays (after an overflow and recapture too) must reproduce the eager loss and gradients."""
+    kw = dict(n_gauss=12000, capacity=4096) if overflow else {}
+    with torch.cuda.stream(torch.cuda.Stream()):
+        _graph_step_body(ssim_lambda=0.2, **kw)
+
+
+def _graph_step_body(n_gauss=4000, capacity=None, ssim_lambda=0.0):
     from dn_splatter_b200.graph_step import GraphedTrainStep
     from dn_splatter_b200.losses import DepthLossType
     from dn_splatter_b200.rasterize import DnrCapacityError
@@ -271,8 +281,8 @@ def _graph_step_body(n_gauss=4000, capacity=None):
     for c in cams:
         c.camera_to_worlds = c.camera_to_worlds.cpu()
     batch = {k: v.cuda() for k, v in _batch(128, 160).items()}
-    kw = dict(use_depth_loss=True, depth_lambda=0.2, depth_loss_type=DepthLossType.EdgeAwareLogL1, ssim_lambda=0.0,
-              sync_free=True)
+    kw = dict(use_depth_loss=True, depth_lambda=0.2, depth_loss_type=DepthLossType.EdgeAwareLogL1,
+              ssim_lambda=ssim_lambda, sync_free=True)
     m = _model(params, **kw)
     bucket = m.enable_flat_grads()
     eager, counts = {}, {}
