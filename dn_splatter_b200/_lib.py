@@ -91,6 +91,21 @@ class DnrMcField(C.Structure):
                 ("spacing", _f)]
 
 
+class DnrPoissonGrid(C.Structure):
+    """Mirror of struct DnrPoissonGrid (include/dnr.h)."""
+
+    _fields_ = [("origin", _f * 3), ("cell", _f), ("depth", _i), ("reserved", _i)]
+
+
+class DnrGridDesc(C.Structure):
+    """Mirror of struct DnrGridDesc (include/dnr.h)."""
+
+    _fields_ = [("origin", _f * 3), ("cell", _f), ("dims", C.c_int32 * 3), ("channels", _i)]
+
+
+POISSON_MIN_DEPTH, POISSON_MAX_DEPTH, POISSON_MAX_CYCLES = 4, 10, 100
+
+
 POINTER_FIELDS = {n for n, t in DnrArgs._fields_ if t is _p}
 
 _lib: Optional[C.CDLL] = None
@@ -105,6 +120,7 @@ KERNELS_PER_CALL = {
     "dnr_grad_zero": (1, 0),
     "dnr_knn_build": (2, 1), "dnr_knn_query": (1, 0), "dnr_density": (1, 0), "dnr_ray_densities": (1, 0),
     "dnr_tsdf_integrate": (1, 0), "dnr_mc_count": (1, 6), "dnr_mc_emit": (2, 0),
+    "dnr_grid_sample": (1, 0),
 }
 LAUNCHES = {"handwritten": 0, "cub": 0}
 DEBUG_CAPTURE = os.environ.get("DNR_DEBUG_CAPTURE") == "1"
@@ -229,6 +245,18 @@ def load():
     lib.dnr_mc_emit.restype = C.c_int
     lib.dnr_mc_emit.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
                                 C.c_void_p]
+    lib.dnr_poisson_splat_workspace_bytes.restype = C.c_int64
+    lib.dnr_poisson_splat_workspace_bytes.argtypes = [C.c_void_p, C.c_int64]
+    lib.dnr_poisson_splat.restype = C.c_int
+    lib.dnr_poisson_splat.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_poisson_solve_workspace_bytes.restype = C.c_int64
+    lib.dnr_poisson_solve_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
+    lib.dnr_poisson_solve.restype = C.c_int
+    lib.dnr_poisson_solve.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_float, C.c_float, C.c_int32, C.c_void_p, C.c_int64,
+                                      C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_grid_sample.restype = C.c_int
+    lib.dnr_grid_sample.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
     lib.dnr_ssim_bwd.restype = C.c_int
     lib.dnr_ssim_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
@@ -248,7 +276,8 @@ EXPORTS = (
     "dnr_raster_bwd", "dnr_project_bwd", "dnr_loss_fwd", "dnr_loss_bwd", "dnr_scale_loss_fwd", "dnr_scale_loss_bwd",
     "dnr_l1_fwd", "dnr_l1_bwd", "dnr_u8_to_f32", "dnr_ssim_fwd", "dnr_ssim_bwd", "dnr_ssim_fwd_ex", "dnr_ssim_bwd_ex", "dnr_photometric_fwd", "dnr_photometric_bwd", "dnr_adam_step", "dnr_adam_step_reduce", "dnr_grad_zero", "dnr_knn_workspace_bytes", "dnr_knn_build", "dnr_knn_query",
     "dnr_density", "dnr_ray_densities", "dnr_tsdf_integrate", "dnr_mc_count_workspace_bytes", "dnr_mc_count",
-    "dnr_mc_emit_workspace_bytes", "dnr_mc_emit",
+    "dnr_mc_emit_workspace_bytes", "dnr_mc_emit", "dnr_poisson_splat_workspace_bytes", "dnr_poisson_splat",
+    "dnr_poisson_solve_workspace_bytes", "dnr_poisson_solve", "dnr_grid_sample",
 )
 
 

@@ -28,6 +28,7 @@ SOURCES = {
     "knn.cu": ["-fmad=false"],
     "density.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],
+    "poisson.cu": [],
 }
 
 

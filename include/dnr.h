@@ -379,6 +379,47 @@ int64_t dnr_mc_emit_workspace_bytes(const int64_t* counts_host);
 int dnr_mc_emit(const DnrMcField* field, const void* count_ws, const int64_t* counts_host, void* ws, int64_t ws_bytes,
                 float* vertices, int32_t* faces, float* colors, void* stream);
 
+/* ---- Screened Poisson reconstruction (Python surface: dn_splatter_b200.poisson; the discrete system is stated in
+ * csrc/poisson.cu and DESIGN.md §2 (6)).  Dense grid of R = 2^depth cells per axis over a cube; chi lives at the cell
+ * centres origin + (index + 0.5) * cell, node (i, j, k) at (i * R + j) * R + k. */
+#define DNR_POISSON_MIN_DEPTH 4
+#define DNR_POISSON_MAX_DEPTH 10
+#define DNR_POISSON_MAX_CYCLES 100
+typedef struct DnrPoissonGrid {
+  float origin[3]; /* corner of cell (0, 0, 0) */
+  float cell;      /* finest cell edge */
+  int32_t depth;   /* DNR_POISSON_MIN_DEPTH..DNR_POISSON_MAX_DEPTH */
+  int32_t reserved;
+} DnrPoissonGrid;
+/* Sorts the n oriented samples (points, normals [n,3]; colors [n,3] or NULL) by finest cell and gathers, per node:
+ * screen [R^3] = S (sum of a_p * trilinear weight), faces [3,R^3] = the MAC face grids of the weighted normals (x, y,
+ * z; face n lies between cell n and its +axis neighbour, the last one per axis is the wall and is 0), density
+ * [(R/4)^3] = the count splat sum-restricted two levels, color_grid [(R/4)^3,4] = {sum a_p w c_p (rgb), sum a_p w} at
+ * that level (NULL iff colors is NULL; the colour at a point is the ratio of the interpolated sums), weights [n] = a_p in input order (or NULL), area_scale [1] = 16 * mean(1 / rho).
+ * Deterministic, no host synchronisation.  n <= 2^31-1. */
+int64_t dnr_poisson_splat_workspace_bytes(const DnrPoissonGrid* grid, int64_t n_points);
+int dnr_poisson_splat(const DnrPoissonGrid* grid, const float* points, const float* normals, const float* colors,
+                      int64_t n_points, void* ws, int64_t ws_bytes, float* screen, float* faces, float* density,
+                      float* color_grid, float* weights, float* area_scale, void* stream);
+/* Solves (-Lap + screen_weight * S) chi = -div V (Neumann walls; mean(chi) = 0 when screen_weight == 0) by multigrid
+ * V-cycles until ||b - A chi|| / ||b|| <= tol or max_cycles.  residual_host[0..cycles] (HOST) receives the relative
+ * residual before the first and after every cycle, *cycles_host the cycle count; one host read per cycle. */
+int64_t dnr_poisson_solve_workspace_bytes(const DnrPoissonGrid* grid, int32_t max_cycles);
+int dnr_poisson_solve(const DnrPoissonGrid* grid, const float* screen, const float* faces, float screen_weight, float tol,
+                      int32_t max_cycles, void* ws, int64_t ws_bytes, float* chi, float* residual_host,
+                      int32_t* cycles_host, void* stream);
+/* Cell-centred grid [dims[0], dims[1], dims[2], channels]: node (i, j, k) sits at origin + (index + 0.5) * cell. */
+typedef struct DnrGridDesc {
+  float origin[3];
+  float cell;
+  int32_t dims[3];
+  int32_t channels;
+} DnrGridDesc;
+/* out[n, channels] = trilinear interpolation of the grid at points [n,3]; coordinates past the outer node centres are
+ * clamped to them. */
+int dnr_grid_sample(const DnrGridDesc* grid, const float* values, const float* points, int64_t n_points, float* out,
+                    void* stream);
+
 #ifdef __cplusplus
 }
 #endif

@@ -11,6 +11,10 @@ Rows (one JSON line each):
               (GraphedTrainStep + FusedAdam) with camera optimisation off vs SO3xR3
   mesh        TSDF fusion of 200 ring views at 1920x1080 into a 512^3 grid over the scene cube (render + integrate, and
               integrate alone, from CUDA events), marching cubes of that volume, export_marching_cubes_mesh at 256^3
+  poisson     export_dn_poisson_mesh on the same scene and views at depth 9 and 10 with CUDA-event stage times (render +
+              back-project, sort + splat, solve and its cycle count, extract, trim + write), the multigrid's algorithmic
+              bytes per cycle and the smoother's share of 3.35 TB/s (red-black kernels timed by torch.profiler in a
+              separate solve), and export_gaussians_poisson_mesh at depth 9
 Each row also checks agreement with the reference path (max abs / rel error), so a faster-but-wrong kernel is visible.
 """
 import argparse
@@ -324,9 +328,95 @@ def bench_mesh():
     emit(row)
 
 
+def multigrid_bytes(depth):
+    """Algorithmic bytes of one V-cycle of dnr_poisson_solve, from the grid size: per node of every level but the 4^3
+    coarsest, 2 + 2 red-black sweeps (each sweep reads chi once, b and S once and writes chi once: 20 B), the residual
+    restriction (chi, b, S: 12 B, plus 1/8 node written), the coarse chi cleared and the prolongation (read chi, write
+    chi, 1/8 node read: 8.5 B); plus the finest-level residual norm (12 B)."""
+    R = 1 << depth
+    levels = [(R >> l) ** 3 for l in range(depth - 2)]
+    smooth = 4 * 20 * sum(levels)
+    return {"smoother": smooth, "total": smooth + sum(n * (12 + 0.5 + 0.5 + 8.5) for n in levels) + 12 * levels[0]}
+
+
+def bench_poisson():
+    """poisson.py on the bench scene, the `dn` exporter's stages one after another as export_dn_poisson_mesh runs them."""
+    import subprocess
+    import tempfile
+
+    from dn_splatter_b200.cameras import Cameras
+    from dn_splatter_b200.dn_model import DNSplatterModelConfig
+    from dn_splatter_b200.mesh import marching_cubes, write_ply
+    from dn_splatter_b200.poisson import (DEFAULT_POINT_WEIGHT, dn_point_cloud, export_gaussians_poisson_mesh, grid_sample,
+                                          poisson_grid, poisson_solve, poisson_splat, trim_low_density)
+    from dn_splatter_b200.synthetic import make_scene, ring_cameras
+
+    W, H, n_views, total = 1920, 1080, 200, 2_000_000
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip().splitlines()[0]
+    m = DNSplatterModelConfig(random_init=True, num_random=16, background_color="black", sync_free=True).setup(device="cuda")
+    m.load_gaussians(make_scene(args.n, seed=0))
+    m.step = 30000
+    cams = [Cameras(c["c2w"][None], c["fx"], c["fy"], c["cx"], c["cy"], W, H) for c in ring_cameras(n_views, W, H)]
+    dn_point_cloud(m, cams[:8], total_points=total // 25)  # warm-up: captures the forward graphs
+    ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
+    with tempfile.TemporaryDirectory() as tmp:
+        for depth in (9, 10):
+            row = {"row": "poisson", "card": card, "n_gauss": args.n, "views": n_views, "resolution": f"{W}x{H}",
+                   "exporter": "dn", "depth": depth, "total_points": total}
+            e = [ev() for _ in range(6)]
+            torch.cuda.synchronize()
+            e[0].record()
+            pts, nrm, col = dn_point_cloud(m, cams, total_points=total)
+            e[1].record()
+            grid = poisson_grid(pts, depth)
+            sp = poisson_splat(pts, nrm, col, grid)
+            e[2].record()
+            sigma = DEFAULT_POINT_WEIGHT * float(sp["area_scale"])
+            chi, hist = poisson_solve(grid, sp["screen"], sp["faces"], sigma)
+            e[3].record()
+            R, h, R4 = grid.R, grid.cell, grid.R // 4
+            chi = chi.view(R, R, R)
+            iso = float((grid_sample(chi, grid.origin, h, pts).double() * sp["weights"].double()).sum() / pts.shape[0])
+            mesh = marching_cubes(chi, iso, [o + 0.5 * h for o in grid.origin], h)
+            dens = grid_sample(sp["density"].view(R4, R4, R4), grid.origin, 4 * h, mesh.vertices)
+            cw = grid_sample(sp["colors"].view(R4, R4, R4, 4), grid.origin, 4 * h, mesh.vertices)
+            mesh = mesh._replace(colors=cw[:, :3] / cw[:, 3:].clamp_min(1e-30))
+            e[4].record()
+            write_ply(os.path.join(tmp, "dn.ply"), trim_low_density(mesh, dens))
+            e[5].record()
+            torch.cuda.synchronize()
+            for k, name in enumerate(("render_backproject", "sort_splat", "solve", "extract", "trim_write")):
+                row[f"{name}_ms"] = e[k].elapsed_time(e[k + 1])
+            row["samples"], row["cycles"], row["residual"] = int(pts.shape[0]), len(hist) - 1, hist[-1]
+            row["triangles"] = int(mesh.faces.shape[0])
+            nbytes = multigrid_bytes(depth)
+            row["bytes_per_cycle"], row["smoother_bytes_per_cycle"] = nbytes["total"], nbytes["smoother"]
+            row["solve_gb_s"] = nbytes["total"] * row["cycles"] / (row["solve_ms"] * 1e-3) / 1e9
+            del chi, mesh, dens, cw
+            with torch.profiler.profile(activities=[torch.profiler.ProfilerActivity.CUDA]) as prof:
+                _, hist2 = poisson_solve(grid, sp["screen"], sp["faces"], sigma)
+                torch.cuda.synchronize()
+            us = sum(getattr(k, "device_time_total", getattr(k, "cuda_time_total", 0.0))
+                     for k in prof.key_averages() if "rbgs_kernel" in k.key)
+            row["smoother_ms"] = us / 1e3
+            row["smoother_gb_s"] = nbytes["smoother"] * (len(hist2) - 1) / (us * 1e-6) / 1e9 if us > 0 else None
+            row["smoother_frac_of_3.35TB_s"] = None if us <= 0 else row["smoother_gb_s"] / 3350.0
+            del sp, pts, nrm, col
+            torch.cuda.empty_cache()
+            emit(row)
+        e0, e1 = ev(), ev()
+        e0.record()
+        g = export_gaussians_poisson_mesh(m, tmp, poisson_depth=9)[0]
+        e1.record()
+        torch.cuda.synchronize()
+        emit({"row": "poisson", "card": card, "n_gauss": args.n, "exporter": "gaussians", "depth": 9,
+              "total_ms": e0.elapsed_time(e1), "triangles": int(g.faces.shape[0])})
+
+
 for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("project_bwd", bench_project_bwd),
                  ("camera_opt", bench_camera_opt), ("knn", bench_knn),
-                 ("render_service", bench_render_service), ("mesh", bench_mesh)):
+                 ("render_service", bench_render_service), ("mesh", bench_mesh), ("poisson", bench_poisson)):
     if args.only and name not in args.only.split(","):
         continue
     try:
