@@ -120,7 +120,7 @@ KERNELS_PER_CALL = {
     "dnr_grad_zero": (1, 0),
     "dnr_knn_build": (2, 1), "dnr_knn_query": (1, 0), "dnr_density": (1, 0), "dnr_ray_densities": (1, 0),
     "dnr_tsdf_integrate": (1, 0), "dnr_mc_count": (1, 6), "dnr_mc_emit": (2, 0),
-    "dnr_grid_sample": (1, 0),
+    "dnr_grid_sample": (1, 0), "dnr_mesh_visibility": (1, 0),
 }
 LAUNCHES = {"handwritten": 0, "cub": 0}
 DEBUG_CAPTURE = os.environ.get("DNR_DEBUG_CAPTURE") == "1"
@@ -257,6 +257,14 @@ def load():
                                       C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dnr_grid_sample.restype = C.c_int
     lib.dnr_grid_sample.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.dnr_mesh_depth_workspace_bytes.restype = C.c_int64
+    lib.dnr_mesh_depth_workspace_bytes.argtypes = [C.c_int64]
+    lib.dnr_mesh_depth.restype = C.c_int
+    lib.dnr_mesh_depth.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                   C.c_float, C.c_float, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.dnr_mesh_visibility.restype = C.c_int
+    lib.dnr_mesh_visibility.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
+                                        C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dnr_ssim_bwd.restype = C.c_int
     lib.dnr_ssim_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
@@ -277,7 +285,8 @@ EXPORTS = (
     "dnr_l1_fwd", "dnr_l1_bwd", "dnr_u8_to_f32", "dnr_ssim_fwd", "dnr_ssim_bwd", "dnr_ssim_fwd_ex", "dnr_ssim_bwd_ex", "dnr_photometric_fwd", "dnr_photometric_bwd", "dnr_adam_step", "dnr_adam_step_reduce", "dnr_grad_zero", "dnr_knn_workspace_bytes", "dnr_knn_build", "dnr_knn_query",
     "dnr_density", "dnr_ray_densities", "dnr_tsdf_integrate", "dnr_mc_count_workspace_bytes", "dnr_mc_count",
     "dnr_mc_emit_workspace_bytes", "dnr_mc_emit", "dnr_poisson_splat_workspace_bytes", "dnr_poisson_splat",
-    "dnr_poisson_solve_workspace_bytes", "dnr_poisson_solve", "dnr_grid_sample",
+    "dnr_poisson_solve_workspace_bytes", "dnr_poisson_solve", "dnr_grid_sample", "dnr_mesh_depth_workspace_bytes",
+    "dnr_mesh_depth", "dnr_mesh_visibility",
 )
 
 

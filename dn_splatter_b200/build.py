@@ -29,6 +29,7 @@ SOURCES = {
     "density.cu": ["-fmad=false"],
     "mesh.cu": ["-fmad=false"],
     "poisson.cu": [],
+    "mesh_eval.cu": ["-fmad=false"],  # visibility counts equal the fp64 oracle's
 }
 
 

@@ -420,6 +420,25 @@ typedef struct DnrGridDesc {
 int dnr_grid_sample(const DnrGridDesc* grid, const float* values, const float* points, int64_t n_points, float* out,
                     void* stream);
 
+/* ---- Mesh evaluation (Python surface: dn_splatter_b200.mesh_eval; rules in csrc/mesh_eval.cu and DESIGN.md §2) ----
+ * Camera blocks are the 16 numbers of dnr_tsdf_integrate's cam_host, {fx, fy, cx, cy, world->camera [3,4] row-major
+ * (OpenCV)}, one per view, in DEVICE memory: float for dnr_mesh_depth, double for dnr_mesh_visibility.
+ *
+ * depth [n_views,H,W] = camera-space z of the nearest hit of the ray through pixel centre (i + 0.5, j + 0.5) with
+ * near <= z <= far, both faces of every triangle, 0 where there is none.  Watertight on shared edges, bit-identical
+ * between runs, no host synchronisation.  Faces with an out-of-range index are skipped. */
+int64_t dnr_mesh_depth_workspace_bytes(int64_t n_faces);
+int dnr_mesh_depth(const float* vertices /* [V,3] */, int32_t n_vertices, const int32_t* faces /* [F,3] */, int64_t n_faces,
+                   const float* cams /* [n_views,16] */, int32_t n_views, int32_t width, int32_t height, float near, float far,
+                   void* ws, int64_t ws_bytes, float* depth, void* stream);
+/* Adds to obs / invalid [n] (int32) the counts of cull_from_one_pose over n_views views, projected in fp64: pz = z + 1e-8,
+ * in frustum = 0 <= px <= W-1, 0 <= py <= H-1, pz > 0; observed = in frustum and pz < rendered + eps (fp32 sum), or in
+ * frustum when rendered is NULL; invalid = in frustum and gt <= 0 (not counted when gt is NULL; invalid may then be NULL).
+ * rendered / gt: [n_views,H,W] float. */
+int dnr_mesh_visibility(const double* points /* [n,3] */, int64_t n_points, const double* cams /* [n_views,16] */,
+                        const float* rendered, const float* gt, int32_t n_views, int32_t width, int32_t height, float eps,
+                        int32_t* obs, int32_t* invalid, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

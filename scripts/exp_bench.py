@@ -15,6 +15,9 @@ Rows (one JSON line each):
               back-project, sort + splat, solve and its cycle count, extract, trim + write), the multigrid's algorithmic
               bytes per cycle and the smoother's share of 3.35 TB/s (red-black kernels timed by torch.profiler in a
               separate solve), and export_gaussians_poisson_mesh at depth 9
+  mesh_eval   the TSDF mesh of that scene against its depth-9 `dn` Poisson mesh, 200 ring views at 1080p: CUDA-event
+              times of depth rendering, visibility counts, subdivision, sampling and nearest neighbours, and the fp64
+              numpy oracle's visibility counts and cKDTree metrics on a subset for scale
 Each row also checks agreement with the reference path (max abs / rel error), so a faster-but-wrong kernel is visible.
 """
 import argparse
@@ -414,9 +417,113 @@ def bench_poisson():
               "total_ms": e0.elapsed_time(e1), "triangles": int(g.faces.shape[0])})
 
 
+def bench_mesh_eval():
+    """mesh_eval.py at a size users run: the bench scene's TSDF mesh (512^3 grid) as pred against its depth-9 `dn`
+    Poisson mesh as gt, the 200 ring views at 1080p; CUDA-event stage times of one cull_mesh + compute_metrics pass
+    (render, visibility, subdivision for both meshes; sampling and nearest neighbours), and the fp64 numpy oracle's
+    visibility counts and cKDTree on a subset for scale."""
+    import subprocess
+    import time
+
+    import numpy as np
+
+    from dn_splatter_b200 import mesh_eval as ME
+    from dn_splatter_b200.cameras import Cameras
+    from dn_splatter_b200.dn_model import DNSplatterModelConfig
+    from dn_splatter_b200.mesh import TSDFVolume, TriangleMesh
+    from dn_splatter_b200.poisson import dn_point_cloud, poisson_reconstruct, trim_low_density
+    from dn_splatter_b200.render_service import ViewRenderer
+    from dn_splatter_b200.synthetic import make_scene, ring_cameras
+    from oracle import mesh_eval_ref as R
+
+    W, H, n_views, chunk = 1920, 1080, 200, 16
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip().splitlines()[0]
+    m = DNSplatterModelConfig(random_init=True, num_random=16, background_color="black", sync_free=True).setup(device="cuda")
+    m.load_gaussians(make_scene(args.n, seed=0))
+    m.step = 30000
+    cams = [Cameras(c["c2w"][None], c["fx"], c["fy"], c["cx"], c["cy"], W, H) for c in ring_cameras(n_views, W, H)]
+    vol = TSDFVolume(((-5.0, -5.0, -5.0), (5.0, 5.0, 5.0)), voxel_size=10.0 / 512, sdf_trunc=3 * 10.0 / 512)
+    for idx, maps in ViewRenderer(m, keys=("rgb", "depth"), to_host=False).render(cams):
+        vol.integrate(maps["depth"], maps["rgb"], cams[idx])
+    pred = vol.extract_mesh()
+    del vol
+    pts, nrm, col = dn_point_cloud(m, cams, total_points=2_000_000)
+    gt, dens = poisson_reconstruct(pts, nrm, col, depth=9)
+    gt = trim_low_density(gt, dens)
+    del pts, nrm, col, dens, m
+    torch.cuda.empty_cache()
+    row = {"row": "mesh_eval", "card": card, "n_gauss": args.n, "views": n_views, "resolution": f"{W}x{H}",
+           "pred_triangles": int(pred.faces.shape[0]), "gt_triangles": int(gt.faces.shape[0])}
+    ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
+    ME.render_mesh_depth(pred, cams[:2])  # warm-up
+    times = {"render_ms": 0.0, "visibility_ms": 0.0, "subdivide_ms": 0.0}
+    culled = {}
+    for tag, mesh in (("pred", pred), ("gt", gt)):
+        e = [ev() for _ in range(2)]
+        e[0].record()
+        v, f = ME._mesh_on(mesh, "cuda", torch.float64)
+        v, f = ME.remove_unreferenced(v, f)
+        sub = ME.subdivide_to_size(TriangleMesh(v, f, None))
+        e[1].record()
+        torch.cuda.synchronize()
+        times["subdivide_ms"] += e[0].elapsed_time(e[1])
+        row[f"{tag}_subdivided_triangles"], row[f"{tag}_subdivided_vertices"] = int(sub.faces.shape[0]), int(sub.vertices.shape[0])
+        v32, f32 = v.float().contiguous(), f.to(torch.int32).contiguous()
+        cams32 = ME.camera_blocks(cams, torch.float32)
+        obs = torch.zeros(sub.vertices.shape[0], dtype=torch.int32, device="cuda")
+        inv = torch.zeros_like(obs)
+        for c0 in range(0, n_views, chunk):
+            c1 = min(c0 + chunk, n_views)
+            e = [ev() for _ in range(3)]
+            e[0].record()
+            depth = ME._depth_call(v32, f32, cams32[c0:c1].contiguous(), W, H, 0.01, 10.0)
+            e[1].record()
+            o, i = ME.visibility_counts(sub.vertices, cams[c0:c1], depth, depth, chunk=c1 - c0)  # rendered depth as gt depth
+            obs += o
+            inv += i
+            e[2].record()
+            torch.cuda.synchronize()
+            times["render_ms"] += e[0].elapsed_time(e[1])
+            times["visibility_ms"] += e[1].elapsed_time(e[2])
+        keep = ME.keep_faces(obs, inv, sub.faces)
+        culled[tag] = TriangleMesh(*ME.remove_unreferenced(sub.vertices, sub.faces[keep]), None)
+        row[f"{tag}_culled_triangles"] = int(keep.sum())
+        if tag == "pred":  # the oracle's host path on the first views, for scale
+            sv = sub.vertices.cpu().numpy()
+            dm = depth.cpu().numpy()
+            bl = [ME.camera_blocks(cams[k:k + 1], torch.float64)[0].cpu().numpy() for k in range(c0, c0 + 2)]
+            t0 = time.perf_counter()
+            ro, ri = R.visibility_counts(sv, bl, W, H, dm[:2], dm[:2])
+            row["oracle_visibility_ms_per_view"] = (time.perf_counter() - t0) / 2 * 1e3
+            o2, i2 = ME.visibility_counts(sub.vertices, cams[c0:c0 + 2], depth[:2], depth[:2])
+            row["visibility_equals_oracle"] = bool(np.array_equal(o2.cpu().numpy(), ro) and np.array_equal(i2.cpu().numpy(), ri))
+    row.update(times)
+    g = torch.Generator(device="cuda").manual_seed(0)
+    e = [ev() for _ in range(3)]
+    e[0].record()
+    n_p, n_g = int(ME.mesh_area(culled["pred"]) * 1e4), int(ME.mesh_area(culled["gt"]) * 1e4)
+    pp, pn = ME.sample_surface(culled["pred"], n_p, g)
+    gp, gn = ME.sample_surface(culled["gt"], n_g, g)
+    e[1].record()
+    met = ME.metrics_from_samples(pp, pn, gp, gn)
+    e[2].record()
+    torch.cuda.synchronize()
+    row["sample_ms"], row["nn_metrics_ms"] = e[0].elapsed_time(e[1]), e[1].elapsed_time(e[2])
+    row["pred_samples"], row["gt_samples"] = n_p, n_g
+    row["nn_queries_per_s"] = (n_p + n_g) / (row["nn_metrics_ms"] * 1e-3)
+    row["metrics"] = met
+    sub_n = min(100_000, n_p, n_g)
+    t0 = time.perf_counter()
+    R.mesh_metrics(pp[:sub_n].cpu().numpy(), pn[:sub_n].cpu().numpy(), gp[:sub_n].cpu().numpy(), gn[:sub_n].cpu().numpy())
+    row["oracle_ckdtree_metrics_s_per_100k"] = time.perf_counter() - t0
+    emit(row)
+
+
 for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("project_bwd", bench_project_bwd),
                  ("camera_opt", bench_camera_opt), ("knn", bench_knn),
-                 ("render_service", bench_render_service), ("mesh", bench_mesh), ("poisson", bench_poisson)):
+                 ("render_service", bench_render_service), ("mesh", bench_mesh), ("poisson", bench_poisson),
+                 ("mesh_eval", bench_mesh_eval)):
     if args.only and name not in args.only.split(","):
         continue
     try:
