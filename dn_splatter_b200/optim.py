@@ -155,10 +155,14 @@ class FusedAdam(torch.optim.Optimizer):
     @torch.no_grad()
     def reference_step(self):
         """The kernel's arithmetic restated in torch, operation for operation (csrc/adam.cu: adam_one) — used ONLY by the
-        CPU test that pins the update rule against torch.optim.Adam; never called by the product path."""
+        CPU tests that pin the update rule (against torch.optim.Adam, and the kernel against it bit for bit); never called
+        by the product path."""
         for (p, g, m, v, lr, eps, bc1, bc2s, b1, b2) in self._segments():
             f = lambda x: torch.tensor(x, dtype=torch.float32)
             m.copy_(m + f(1.0 - b1) * (g - m))
             v.copy_(f(b2) * v + f(1.0 - b2) * g * g)
-            denom = v.sqrt() / f(bc2s) + f(eps)
+            # sqrtf is correctly rounded; torch's CPU float32 sqrt (a vector-math library) is not always (1 ulp off on
+            # ~0.6 % of inputs with AVX-512).  The float64 sqrt rounded to float32 is: the double rounding of a square
+            # root is harmless at 53 >= 2 * 24 + 2 bits.
+            denom = v.double().sqrt().float() / f(bc2s) + f(eps)
             p.copy_(p - f(lr / bc1) * (m / denom))

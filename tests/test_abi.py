@@ -112,6 +112,79 @@ def test_argument_errors_of_the_8f_entry_points(lib):
     assert lib.dnr_ray_densities(one, 5, one, 16, one, one, one, one, one, 10, 20, 3.0, one, one, one, None) == -3  # 21 samples only
 
 
+def _reduce_call(lib, break_one):
+    """dnr_adam_step_reduce on fake 16-byte-aligned addresses (never dereferenced): a valid call at world 3, rank 1 with
+    one field broken by `break_one(segs, widths, peers)`, which returns the arguments to pass instead when it replaces
+    one (n_segs).  Every case must fail a host check, so nothing is launched."""
+    segs = (L.DnrAdamSeg * 2)()
+    widths = (C.c_int32 * 2)(3, 45)
+    pr = L.DnrPeerReduce()
+    pr.world, pr.rank, pr.n_gauss = 3, 1, 8
+    for k in range(3):
+        pr.peer_flat[k], pr.peer_touched[k] = 0x1000000 * (k + 1), 0x1000000 * (k + 1) + 0x800000
+    pr.mask = 0x9000000
+    for i, (off, w) in enumerate(((0, 3), (24, 45))):  # segment offsets in floats, multiples of 4
+        segs[i].p, segs[i].m, segs[i].v = 0x10000000 + 0x100000 * i, 0x20000000 + 0x100000 * i, 0x30000000 + 0x100000 * i
+        segs[i].g = pr.peer_flat[1] + 4 * off
+        segs[i].n, segs[i].lr, segs[i].eps, segs[i].bc1, segs[i].bc2_sqrt = 8 * w, 1e-3, 1e-15, 0.1, 0.03
+    n_segs = break_one(segs, widths, pr)
+    return lib.dnr_adam_step_reduce(C.cast(segs, C.c_void_p), C.cast(widths, C.c_void_p), 2 if n_segs is None else n_segs,
+                                    0.9, 0.999, C.byref(pr), None)
+
+
+def _set(obj, **kw):
+    for k, v in kw.items():
+        setattr(obj, k, v)
+
+
+REDUCE_ARGUMENT_ERRORS = {
+    "null_segs": (-1, None),
+    "null_widths": (-1, None),
+    "null_peers": (-1, None),
+    "n_segs_0": (-2, lambda s, w, p: 0),
+    "n_segs_17": (-2, lambda s, w, p: 17),
+    "world_0": (-2, lambda s, w, p: _set(p, world=0)),
+    "world_9": (-2, lambda s, w, p: _set(p, world=9)),
+    "rank_-1": (-2, lambda s, w, p: _set(p, rank=-1)),
+    "rank_eq_world": (-2, lambda s, w, p: _set(p, rank=3)),
+    "n_gauss_0": (-2, lambda s, w, p: _set(p, n_gauss=0)),
+    "null_mask_at_world_3": (-1, lambda s, w, p: _set(p, mask=None)),
+    "null_peer_flat_0": (-1, lambda s, w, p: p.peer_flat.__setitem__(0, None)),
+    "null_peer_flat_2": (-1, lambda s, w, p: p.peer_flat.__setitem__(2, None)),
+    "null_peer_touched_2": (-1, lambda s, w, p: p.peer_touched.__setitem__(2, None)),
+    "null_p": (-1, lambda s, w, p: _set(s[1], p=None)),
+    "width_0": (-2, lambda s, w, p: w.__setitem__(1, 0)),
+    "n_not_a_multiple_of_width": (-2, lambda s, w, p: _set(s[1], n=8 * 45 + 1)),
+    "n_over_width_is_not_n_gauss": (-2, lambda s, w, p: _set(s[1], n=9 * 45)),
+    "n_at_2_pow_32": (-2, lambda s, w, p: (_set(p, n_gauss=1 << 30), _set(s[0], n=3 << 30), w.__setitem__(1, 4),
+                                           _set(s[1], n=1 << 32)) and None),
+    "g_below_peer_flat_rank": (-2, lambda s, w, p: _set(s[0], g=p.peer_flat[1] - 16)),
+    "g_offset_1_float": (-2, lambda s, w, p: _set(s[1], g=s[1].g + 4)),
+    "g_offset_2_floats": (-2, lambda s, w, p: _set(s[1], g=s[1].g + 8)),
+    "g_offset_3_floats": (-2, lambda s, w, p: _set(s[1], g=s[1].g + 12)),
+    "p_misaligned": (-2, lambda s, w, p: _set(s[1], p=s[1].p + 4)),
+    "m_misaligned": (-2, lambda s, w, p: _set(s[1], m=s[1].m + 8)),
+    "v_misaligned": (-2, lambda s, w, p: _set(s[0], v=s[0].v + 12)),
+    "bc1_0": (-2, lambda s, w, p: _set(s[1], bc1=0.0)),
+    "bc1_negative": (-2, lambda s, w, p: _set(s[0], bc1=-0.5)),
+    "bc1_nan": (-2, lambda s, w, p: _set(s[0], bc1=float("nan"))),
+}
+
+
+@pytest.mark.parametrize("case", list(REDUCE_ARGUMENT_ERRORS))
+def test_argument_errors_of_adam_step_reduce(lib, case):
+    """Host checks of dnr_adam_step_reduce, each from a valid call with exactly one field broken: a negative code before
+    any CUDA call."""
+    want, brk = REDUCE_ARGUMENT_ERRORS[case]
+    if brk is None:  # a NULL array or struct
+        segs, widths, pr = (L.DnrAdamSeg * 1)(), (C.c_int32 * 1)(3), L.DnrPeerReduce()
+        args = [C.cast(segs, C.c_void_p), C.cast(widths, C.c_void_p), 1, 0.9, 0.999, C.byref(pr), None]
+        args[{"null_segs": 0, "null_widths": 1, "null_peers": 5}[case]] = None
+        assert lib.dnr_adam_step_reduce(*args) == want
+        return
+    assert _reduce_call(lib, brk) == want
+
+
 def test_product_path_fails_loudly_without_cuda():
     import torch
 

@@ -92,6 +92,35 @@ def _grad_zero_mirror(seg, flags, width, dense, chunk=256):
     return out, stores
 
 
+def grad_zero_mirror_vec(seg, flags, width, dense):
+    """_grad_zero_mirror without the per-float4 Python loop (for segments of millions of floats): chunks of 256 Gaussians
+    start on float4 boundaries, so float4 q of the padded segment is stored iff the segment is dense or a Gaussian among
+    those of its four elements (the last one standing in for the padding) is flagged."""
+    n = flags.size
+    q4 = np.arange((n * width + 3) // 4, dtype=np.int64) * 4
+    hit = np.full(q4.size, bool(dense))
+    if not dense:
+        for r in range(4):
+            hit |= flags[np.minimum((q4 + r) // width, n - 1)] != 0
+    out = seg.copy()
+    out[:4 * q4.size].reshape(-1, 4)[hit] = 0.0
+    return out, int(hit.sum())
+
+
+@pytest.mark.parametrize("width", [1, 2, 3, 4, 45, 4096])
+@pytest.mark.parametrize("n_gauss", [1, 255, 256, 257, 600])
+def test_vectorised_grad_zero_mirror_equals_the_loop(width, n_gauss):
+    rng = np.random.default_rng(width * 7 + n_gauss)
+    flags = (rng.random(n_gauss) < 0.02).astype(np.uint8) * rng.choice(np.array([1, 0x80, 0xff], np.uint8), n_gauss)
+    flags[-1] = 2
+    if n_gauss == 600:
+        flags[256:512] = 0  # a chunk without flags
+    seg = rng.uniform(1, 2, (n_gauss * width + 3) & ~3).astype(np.float32)
+    for dense in (False, True):
+        a, b = _grad_zero_mirror(seg, flags, width, dense), grad_zero_mirror_vec(seg, flags, width, dense)
+        assert np.array_equal(a[0], b[0]) and a[1] == b[1]
+
+
 @pytest.mark.parametrize("width", [1, 3, 4, 45])
 @pytest.mark.parametrize("n_gauss", [37, 600])
 def test_grad_zero_clears_every_flagged_row_and_stays_in_the_padded_segment(width, n_gauss):
