@@ -11,8 +11,6 @@ LIB_PATH = os.path.join(HERE, "libdnr_b200.so")
 
 FLAG_ACTIVATED, FLAG_ANTIALIASED, FLAG_NORMALS, FLAG_ACCUMULATE, FLAG_EXACT_LISTS = 1, 2, 4, 8, 16
 FLAG_HOST_CAMERA = 32
-FLAG_COMPACT_BWD = 64
-FLAG_TOUCHED_BWD = 128
 FLAG_PERSISTENT_WS = 256
 LOSS_FUSED_BWD, LOSS_IMG_U8, LOSS_NORMAL_U8, LOSS_EDGE_FROM_IMAGE = 1, 2, 4, 8
 REC_FLOATS, REC_FLOATS_N, GRAD_FLOATS = 12, 16, 16
@@ -43,8 +41,8 @@ class DnrArgs(C.Structure):
         ("gt_depth", _p), ("gt_normal", _p), ("gt_rgb", _p), ("loss_partials", _p), ("v_loss", _p),
         ("depth_lambda", _f), ("depth_tolerance", _f), ("depth_loss_type", _i), ("use_normal_loss", _i),
         ("host_cam", _f * 32),
-        ("depth_order", _p),
-        ("loss_flags", C.c_uint32), ("variant", _i), ("gt_image", _p), ("v_l1", _p), ("touched", _p), ("stats", _p),
+        ("reserved2", _p),
+        ("loss_flags", C.c_uint32), ("reserved3", _i), ("gt_image", _p), ("v_l1", _p), ("touched", _p), ("stats", _p),
         ("v_viewmat", _p),
     ]
 
@@ -268,8 +266,6 @@ def load():
     lib.dnr_ssim_bwd.restype = C.c_int
     lib.dnr_ssim_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
-    lib.dnr_depth_order_ptr.restype = C.c_void_p
-    lib.dnr_depth_order_ptr.argtypes = [C.c_void_p, C.c_int32]
     lib.dnr_bin_scan_workspace_bytes.restype = C.c_size_t
     lib.dnr_bin_scan_workspace_bytes.argtypes = [C.c_int32]
     lib.dnr_bin_sort_workspace_bytes.restype = C.c_size_t
@@ -280,7 +276,7 @@ def load():
 
 EXPORTS = (
     "dnr_version", "dnr_error_string", "dnr_project_fwd", "dnr_bin_scan_workspace_bytes", "dnr_bin_scan",
-    "dnr_bin_sort_workspace_bytes", "dnr_bin_sort", "dnr_depth_order_ptr", "dnr_raster_fwd", "dnr_finalize_fwd", "dnr_normal_from_depth",
+    "dnr_bin_sort_workspace_bytes", "dnr_bin_sort", "dnr_raster_fwd", "dnr_finalize_fwd", "dnr_normal_from_depth",
     "dnr_raster_bwd", "dnr_project_bwd", "dnr_loss_fwd", "dnr_loss_bwd", "dnr_scale_loss_fwd", "dnr_scale_loss_bwd",
     "dnr_l1_fwd", "dnr_l1_bwd", "dnr_u8_to_f32", "dnr_ssim_fwd", "dnr_ssim_bwd", "dnr_ssim_fwd_ex", "dnr_ssim_bwd_ex", "dnr_photometric_fwd", "dnr_photometric_bwd", "dnr_adam_step", "dnr_adam_step_reduce", "dnr_grad_zero", "dnr_knn_workspace_bytes", "dnr_knn_build", "dnr_knn_query",
     "dnr_density", "dnr_ray_densities", "dnr_tsdf_integrate", "dnr_mc_count_workspace_bytes", "dnr_mc_count",

@@ -303,11 +303,6 @@ extern "C" size_t dnr_bin_scan_workspace_bytes(int32_t n_gauss) {
   return carve_scan(nullptr, n_gauss).total;
 }
 
-extern "C" const int32_t* dnr_depth_order_ptr(void* ws_scan, int32_t n_gauss) {
-  if (!ws_scan || n_gauss <= 0) return nullptr;
-  return carve_scan(ws_scan, n_gauss).order;
-}
-
 extern "C" int dnr_bin_scan(const DnrArgs* a, void* stream, int64_t* n_isects_host) {
   if (!a) return DNR_E_NULL;
   if (a->n_gauss <= 0 || a->width <= 0 || a->height <= 0) return DNR_E_SIZE;

@@ -602,108 +602,13 @@ __device__ __forceinline__ void cta_add_viewmat(const float* s_pv, float* v_view
   }
 }
 
-// The 180 B/Gaussian SH-gradient rows are staged in shared memory (stride 45 words: conflict-free) and written
-// by the whole CTA as one contiguous, coalesced stream instead of 45 strided 4-byte stores per thread.
-// COMPACT (DNR_FLAG_COMPACT_BWD, kept for A/B; the touched-flag kernel below is the default): slot s of the grid handles Gaussian depth_order[s]; the visible ones
-// come first in that order, so full CTAs do useful work and the tail CTAs leave after one load.  Rows are then
-// scattered, hence accumulate-only.
-// VIEWMAT (not with COMPACT): also adds d(loss)/d(viewmat) into a.v_viewmat, one CTA reduction at the end; a CTA that
-// leaves early at the __syncthreads_or below has no visible Gaussian and contributes zero.
-template <bool NORMALS, bool COMPACT, bool VIEWMAT = false>
-__global__ void __launch_bounds__(PB_THREADS, 8) project_bwd_kernel(const DnrArgs a) {
-  static_assert(!(COMPACT && VIEWMAT), "the compact path does not compute viewmat gradients");
-  __shared__ float s_rest[PB_THREADS * PB_REST_MAX];
-  __shared__ unsigned char s_vis[PB_THREADS];
-  __shared__ unsigned char s_list[PB_THREADS];
-  __shared__ int s_gid[COMPACT ? PB_THREADS : 1];
-  __shared__ int s_nvis;
-  const int slot = blockIdx.x * PB_THREADS + threadIdx.x;
-  const bool in_range = slot < a.n_gauss;
-  const int i = COMPACT ? (in_range ? a.depth_order[slot] : 0) : slot;  // Gaussian id
-  if (COMPACT) s_gid[threadIdx.x] = i;
-  const bool acc = COMPACT ? true : (a.flags & DNR_FLAG_ACCUMULATE) != 0;
-  const int nrest = a.sh_bases - 1;
-  const int nrow = nrest * 3;
-  const int radius = in_range ? a.radii[i] : 0;
-  const bool visible = radius > 0;
-  s_vis[threadIdx.x] = visible ? 1 : 0;
-  // means2d.grad / .absgrad (what densification reads) are plain outputs, not accumulators: invisible rows are zero in
-  // every mode (the caller hands in uninitialised buffers)
-  if (in_range && !visible) {
-    if (a.v_means2d) { a.v_means2d[i * 2] = 0.f; a.v_means2d[i * 2 + 1] = 0.f; }
-    if (a.v_means2d_abs) { a.v_means2d_abs[i * 2] = 0.f; a.v_means2d_abs[i * 2 + 1] = 0.f; }
-  }
-  float* srow = s_rest + threadIdx.x * PB_REST_MAX;
-  // visible rows are fully written by the SH section below; invisible rows are only read by the dense-overwrite path
-  if (!visible && !acc) {
-#pragma unroll
-    for (int k = 0; k < PB_REST_MAX; ++k) srow[k] = 0.f;
-  }
-  if (acc && !__syncthreads_or(visible ? 1 : 0)) return;  // nothing to accumulate from this CTA
-  float vm[3] = {0, 0, 0}, vq[4] = {0, 0, 0, 0}, vs[3] = {0, 0, 0}, vo = 0.f, vdc[3] = {0, 0, 0};
-  __shared__ float s_pv[VIEWMAT ? 12 * PB_THREADS : 1];
-  float* pv = VIEWMAT ? s_pv + threadIdx.x : nullptr;
-  if constexpr (VIEWMAT) {
-#pragma unroll
-    for (int k = 0; k < 12; ++k) pv[k * PB_THREADS] = 0.f;
-  }
-  if (in_range && !visible && !acc) {
-    for (int k = 0; k < 3; ++k) { a.v_means[i * 3 + k] = 0.f; a.v_scales[i * 3 + k] = 0.f; a.v_sh_dc[i * 3 + k] = 0.f; }
-    for (int k = 0; k < 4; ++k) a.v_quats[i * 4 + k] = 0.f;
-    a.v_opacities[i] = 0.f;
-  }
-  if (visible) project_bwd_gauss<NORMALS, VIEWMAT>(a, i, nrest, srow, vm, vq, vs, vo, vdc, pv);
-  if (!in_range) {
-    // the last CTA's lanes past n_gauss own no row (they only take part in the barriers below)
-  } else if (acc) {
-    for (int k = 0; k < 3; ++k) { a.v_means[i * 3 + k] += vm[k]; a.v_scales[i * 3 + k] += vs[k]; a.v_sh_dc[i * 3 + k] += vdc[k]; }
-    for (int k = 0; k < 4; ++k) a.v_quats[i * 4 + k] += vq[k];
-    a.v_opacities[i] += vo;
-  } else {
-    for (int k = 0; k < 3; ++k) { a.v_means[i * 3 + k] = vm[k]; a.v_scales[i * 3 + k] = vs[k]; a.v_sh_dc[i * 3 + k] = vdc[k]; }
-    for (int k = 0; k < 4; ++k) a.v_quats[i * 4 + k] = vq[k];
-    a.v_opacities[i] = vo;
-  }
-  __syncthreads();
-  if (nrest > 0) {
-    const int g0 = blockIdx.x * PB_THREADS;
-    const int ng = min(PB_THREADS, a.n_gauss - g0);
-    float* out = a.v_sh_rest + (size_t)g0 * nrow;
-    if (!acc) {
-      // dense overwrite: the CTA's rows are one contiguous span of ng*nrow floats
-      for (int e = threadIdx.x; e < ng * nrow; e += PB_THREADS) out[e] = s_rest[(e / nrow) * PB_REST_MAX + e % nrow];
-    } else {
-      // accumulate only the visible rows: compact their indices, then spread (row, element) pairs over the CTA so
-      // the read-modify-writes of different rows overlap (each row is a contiguous 4*nrow-byte span)
-      if (threadIdx.x < 32) {
-        int base = 0;
-        for (int g0l = 0; g0l < PB_THREADS; g0l += 32) {
-          const bool vz = (g0l + threadIdx.x < ng) && s_vis[g0l + threadIdx.x];
-          const unsigned m = __ballot_sync(0xffffffffu, vz);
-          if (vz) s_list[base + __popc(m & ((1u << threadIdx.x) - 1u))] = (unsigned char)(g0l + threadIdx.x);
-          base += __popc(m);
-        }
-        if (threadIdx.x == 0) s_nvis = base;
-      }
-      __syncthreads();
-      const int total = s_nvis * nrow;
-      for (int e = threadIdx.x; e < total; e += PB_THREADS) {
-        const int r = s_list[e / nrow], k = e % nrow;
-        if (COMPACT) a.v_sh_rest[(size_t)s_gid[r] * nrow + k] += s_rest[r * PB_REST_MAX + k];
-        else out[(size_t)r * nrow + k] += s_rest[r * PB_REST_MAX + k];
-      }
-    }
-  }
-  if constexpr (VIEWMAT) cta_add_viewmat(s_pv, a.v_viewmat);
-}
-
-// DNR_FLAG_TOUCHED_BWD: only Gaussians that received a raster gradient are processed (touched[g] != 0, written by
-// dnr_raster_bwd).  On the 1 M-Gaussian / 1080p scene ~40 % are visible but only ~10 % are ever composited before the
-// pixels saturate; the dense kernel above still pays a latency-bound pass over every warp that holds one visible
-// Gaussian.  Here a CTA scans the flags of PB_SCAN consecutive Gaussians (coalesced bytes), compacts the touched ids in
-// shared memory and then runs the per-Gaussian backward with every lane busy; the 180 B SH rows are staged in shared
-// memory and accumulated row by row (each row is a contiguous span).  Accumulate-only: the caller pre-zeroes the
-// gradient buffers (and v_means2d / v_means2d_abs).
+// Only Gaussians that received a raster gradient are processed (touched[g] != 0, written by dnr_raster_bwd).  On the
+// 1 M-Gaussian / 1080p scene ~40 % are visible but only ~10 % are ever composited before the pixels saturate, so a pass
+// with one lane per Gaussian would leave most lanes idle.  Here a CTA scans the flags of PB_SCAN consecutive Gaussians
+// (coalesced bytes), compacts the touched ids in shared memory and then runs the per-Gaussian backward with every lane
+// busy; the 180 B SH rows are staged in shared memory (stride 45 words: conflict-free) and accumulated row by row (each
+// row is a contiguous span).  Accumulate-only: the caller pre-zeroes the gradient buffers (and v_means2d /
+// v_means2d_abs).
 constexpr int PB_SCAN = 1024;
 
 // VIEWMAT: each thread sums its Gaussians' d(loss)/d(viewmat) over the loop; one CTA reduction adds it to a.v_viewmat.
@@ -817,32 +722,16 @@ extern "C" int dnr_project_bwd(const DnrArgs* a, void* stream) {
   const bool normals = (a->flags & DNR_FLAG_NORMALS) != 0;
   if (normals && !hostcam && !a->c2w) return DNR_E_NULL;
   if (a->sh_bases > 16) return DNR_E_OPTION;
-  const int block = PB_THREADS, grid = (a->n_gauss + block - 1) / block;
+  if (!a->touched) return DNR_E_NULL;
+  if (!(a->flags & DNR_FLAG_ACCUMULATE)) return DNR_E_OPTION;  // scattered rows: the caller pre-zeroes and accumulates
+  const int grid = (a->n_gauss + PB_SCAN - 1) / PB_SCAN;
   cudaStream_t s = (cudaStream_t)stream;
-  const bool vmat = a->v_viewmat != nullptr;
-  if (a->flags & DNR_FLAG_TOUCHED_BWD) {
-    if (!a->touched) return DNR_E_NULL;
-    if (!(a->flags & DNR_FLAG_ACCUMULATE)) return DNR_E_OPTION;  // scattered rows: the caller pre-zeroes and accumulates
-    const int tgrid = (a->n_gauss + PB_SCAN - 1) / PB_SCAN;
-    if (vmat) {
-      if (normals) project_bwd_touched_kernel<true, true><<<tgrid, block, 0, s>>>(*a);
-      else project_bwd_touched_kernel<false, true><<<tgrid, block, 0, s>>>(*a);
-    } else {
-      if (normals) project_bwd_touched_kernel<true><<<tgrid, block, 0, s>>>(*a);
-      else project_bwd_touched_kernel<false><<<tgrid, block, 0, s>>>(*a);
-    }
-  } else if (a->flags & DNR_FLAG_COMPACT_BWD) {
-    if (vmat) return DNR_E_OPTION;  // the compact A/B path has no viewmat gradient
-    if (!a->depth_order) return DNR_E_NULL;
-    if (!(a->flags & DNR_FLAG_ACCUMULATE)) return DNR_E_OPTION;  // scattered rows: the caller pre-zeroes and accumulates
-    if (normals) project_bwd_kernel<true, true><<<grid, block, 0, s>>>(*a);
-    else project_bwd_kernel<false, true><<<grid, block, 0, s>>>(*a);
-  } else if (vmat) {
-    if (normals) project_bwd_kernel<true, false, true><<<grid, block, 0, s>>>(*a);
-    else project_bwd_kernel<false, false, true><<<grid, block, 0, s>>>(*a);
+  if (a->v_viewmat != nullptr) {
+    if (normals) project_bwd_touched_kernel<true, true><<<grid, PB_THREADS, 0, s>>>(*a);
+    else project_bwd_touched_kernel<false, true><<<grid, PB_THREADS, 0, s>>>(*a);
   } else {
-    if (normals) project_bwd_kernel<true, false><<<grid, block, 0, s>>>(*a);
-    else project_bwd_kernel<false, false><<<grid, block, 0, s>>>(*a);
+    if (normals) project_bwd_touched_kernel<true><<<grid, PB_THREADS, 0, s>>>(*a);
+    else project_bwd_touched_kernel<false><<<grid, PB_THREADS, 0, s>>>(*a);
   }
   DNR_CHECK_LAUNCH();
   return 0;

@@ -23,8 +23,8 @@
 //
 // Arithmetic.  A thread owns 2 (forward) / 4 (backward) pixels of one column and evaluates them as pairs of scalar fp32
 // operations with explicit rounding (V2 in common.cuh).  The backward's per-record warp reduction of its 16 gradient
-// values goes through a padded shared-memory transpose (4 STS.128 + 16 LDS.32 per lane, no SEL) instead of a
-// 16-SHFL / 30-SEL butterfly (variant bit 0), and is paid once per 128 pixels.
+// values goes through a padded shared-memory transpose (4 STS.128 + 16 LDS.32 per lane, no SEL: fewer instructions than
+// a 16-SHFL / 30-SEL shuffle reduction), and is paid once per 128 pixels.
 #include "common.cuh"
 #include "loss_common.cuh"
 
@@ -333,47 +333,9 @@ __device__ __forceinline__ void fused_loss_grads(const DnrArgs& a, int i, int j,
 }
 
 // ------------------------------------------------------------------------------------------------ backward
-// 16 per-lane values -> per-value warp totals in 16 shuffles (transposing butterfly); on return the lane
-// holds in v[0] the total of value index (lane>>1)&15.  (variant bit 0: kept for A/B timing.)
-__device__ __forceinline__ float butterfly16(float (&v)[16], int lane) {
-  {
-    const bool up = (lane & 16) != 0;
-#pragma unroll
-    for (int k = 0; k < 8; ++k) {
-      const float send = up ? v[k] : v[k + 8];
-      const float keep = up ? v[k + 8] : v[k];
-      v[k] = keep + __shfl_xor_sync(0xffffffffu, send, 16);
-    }
-  }
-  {
-    const bool up = (lane & 8) != 0;
-#pragma unroll
-    for (int k = 0; k < 4; ++k) {
-      const float send = up ? v[k] : v[k + 4];
-      const float keep = up ? v[k + 4] : v[k];
-      v[k] = keep + __shfl_xor_sync(0xffffffffu, send, 8);
-    }
-  }
-  {
-    const bool up = (lane & 4) != 0;
-#pragma unroll
-    for (int k = 0; k < 2; ++k) {
-      const float send = up ? v[k] : v[k + 2];
-      const float keep = up ? v[k + 2] : v[k];
-      v[k] = keep + __shfl_xor_sync(0xffffffffu, send, 4);
-    }
-  }
-  {
-    const bool up = (lane & 2) != 0;
-    const float send = up ? v[0] : v[1];
-    const float keep = up ? v[1] : v[0];
-    v[0] = keep + __shfl_xor_sync(0xffffffffu, send, 2);
-  }
-  return v[0] + __shfl_xor_sync(0xffffffffu, v[0], 1);
-}
-
-// The same totals through a padded shared-memory transpose: no SEL, 4 STS.128 + 16 LDS.32 per lane.  Lane L returns the
-// total of value index L & 15 (both half-warps hold it).  `scr` is the warp's private [32][RED_STRIDE] scratch.
+// 16 per-lane values -> per-value warp totals through a padded shared-memory transpose: no SEL, 4 STS.128 + 16 LDS.32
+// per lane.  Lane L returns the total of value index L & 15 (both half-warps hold it).  `scr` is the warp's private
+// [32][RED_STRIDE] scratch.
 __device__ __forceinline__ float transpose_reduce16(const float (&v)[16], float* scr, int lane) {
   __syncwarp();  // previous reads of the scratch are done
   float4* row = reinterpret_cast<float4*>(scr + lane * RED_STRIDE + (lane >> 4) * 16);
@@ -397,8 +359,7 @@ __device__ __forceinline__ float transpose_reduce16(const float (&v)[16], float*
   return s + __shfl_xor_sync(0xffffffffu, s, 16);
 }
 
-// VARIANT: 0 = shared-memory transpose reduction, 1 = shuffle butterfly
-template <bool NORMALS, int VARIANT>
+template <bool NORMALS>
 __global__ void __launch_bounds__(BWD_THREADS, 9) raster_bwd_kernel(const DnrArgs a, int stiles_x) {
   constexpr int REC = NORMALS ? DNR_REC_FLOATS_N : DNR_REC_FLOATS;
   constexpr int RQ = REC / 4;
@@ -409,7 +370,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 9) raster_bwd_kernel(const DnrArg
   __shared__ __align__(4) unsigned char sidx[CH];
   __shared__ int scnt[NW];
   __shared__ int red_last[NW];
-  __shared__ __align__(16) float red_scr[VARIANT == 0 ? NW * RED_WARP_FLOATS : 4];
+  __shared__ __align__(16) float red_scr[NW * RED_WARP_FLOATS];
 
   const int tid = threadIdx.x, lane = tid & 31, warp = tid >> 5;
   const int shift = a.list_shift;
@@ -512,7 +473,7 @@ __global__ void __launch_bounds__(BWD_THREADS, 9) raster_bwd_kernel(const DnrArg
   // per-lane post-scale of the reduced totals (lane k & 15 owns value k): conic rows 0.5, mean rows -ln2 / ln2 (abs)
   const int vk = lane & 15;
   const float post = (vk == 0 || vk == 1) ? -DNR_LN2 : ((vk == 2 || vk == 3) ? DNR_LN2 : ((vk == 4 || vk == 6) ? 0.5f : 1.0f));
-  float* scr = red_scr + (VARIANT == 0 ? warp * RED_WARP_FLOATS : 0);
+  float* scr = red_scr + warp * RED_WARP_FLOATS;
   unsigned long long walked = 0, kept = 0;
 
   // chunk c covers list positions [chi - n_c, chi), chi = hi - c*CH; slot t <-> position chi-1-t
@@ -620,15 +581,8 @@ __global__ void __launch_bounds__(BWD_THREADS, 9) raster_bwd_kernel(const DnrArg
       float v[16];
 #pragma unroll
       for (int k = 0; k < 16; ++k) v[k] = lo(acc[k]) + hi(acc[k]);
-      if (VARIANT == 0) {
-        const float tot = transpose_reduce16(v, scr, lane) * post;
-        if (lane < 16 && tot != 0.f) atomicAdd(a.grad_records + (size_t)gid * DNR_GRAD_FLOATS + lane, tot);
-      } else {
-        const float tot = butterfly16(v, lane);
-        const int k = (lane >> 1) & 15;
-        const float ps = (k == 0 || k == 1) ? -DNR_LN2 : ((k == 2 || k == 3) ? DNR_LN2 : ((k == 4 || k == 6) ? 0.5f : 1.0f));
-        if ((lane & 1) == 0 && tot != 0.f) atomicAdd(a.grad_records + (size_t)gid * DNR_GRAD_FLOATS + k, tot * ps);
-      }
+      const float tot = transpose_reduce16(v, scr, lane) * post;
+      if (lane < 16 && tot != 0.f) atomicAdd(a.grad_records + (size_t)gid * DNR_GRAD_FLOATS + lane, tot);
       if (a.touched != nullptr && lane == 0) a.touched[gid] = 1;
     }
     __syncthreads();  // stage, sidx and ids_s free for the chunk after next
@@ -695,14 +649,8 @@ extern "C" int dnr_raster_bwd(const DnrArgs* a, void* stream) {
   if (a->n_isects == 0) return 0;
   const dim3 grid(dnr_tiles_x(a), dnr_tiles_y(a));
   const int sx = dnr_stiles_x(a);
-  const bool butterfly = (a->variant & 1) != 0;  // variant bit 0: shuffle-butterfly reduction (A/B timing)
-  if (normals) {
-    if (butterfly) raster_bwd_kernel<true, 1><<<grid, BWD_THREADS, 0, s>>>(*a, sx);
-    else raster_bwd_kernel<true, 0><<<grid, BWD_THREADS, 0, s>>>(*a, sx);
-  } else {
-    if (butterfly) raster_bwd_kernel<false, 1><<<grid, BWD_THREADS, 0, s>>>(*a, sx);
-    else raster_bwd_kernel<false, 0><<<grid, BWD_THREADS, 0, s>>>(*a, sx);
-  }
+  if (normals) raster_bwd_kernel<true><<<grid, BWD_THREADS, 0, s>>>(*a, sx);
+  else raster_bwd_kernel<false><<<grid, BWD_THREADS, 0, s>>>(*a, sx);
   DNR_CHECK_LAUNCH();
   return 0;
 }

@@ -456,8 +456,7 @@ class DNSplatterModel(_ModelBase):
         dual = cfg.rasterize_mode == "antialiased" and cfg.predict_normals
         common = dict(sh_degree=sh_degree_to_use, near_plane=0.01, far_plane=1e10, background=background, c2w=c2w_fixed,
                       exact_lists=cfg.exact_isect_lists, sync_free=cfg.sync_free, fixed_capacity=fixed_capacity,
-                      list_shift=cfg.list_shift, stats=self.__dict__.get("_raster_stats"),
-                      variant=self.__dict__.get("_raster_variant", 0))
+                      list_shift=cfg.list_shift, stats=self.__dict__.get("_raster_stats"))
         params = (self.means, self.quats, self.scales, self.opacities, self.features_dc, self.features_rest, viewmat, K, W, H)
         sink = self._bucket.sink() if (self._bucket is not None and torch.is_grad_enabled()) else None
         out = dn_rasterize(*params, antialiased=cfg.rasterize_mode == "antialiased",

@@ -58,8 +58,8 @@ class FlatGradBucket:
         self.dense_params = {"scales"} & set(self.params)
         # False for configs with other parameter-only loss terms (dn_model.enable_flat_grads)
         self.sparse_ok = True
-        # flags_valid: every non-zero row outside the dense segments is flagged.  Only a flagged backward through sink()
-        # makes the flags valid; a fresh bucket may have been filled by other means.
+        # flags_valid: every non-zero row outside the dense segments is flagged.  Only a backward through sink() after a
+        # zero_() makes the flags valid; a fresh bucket may have been filled by other means.
         self.flags_valid, self._clean = False, False
         _BUCKETS[self.flat.data_ptr()] = self
 
@@ -88,10 +88,10 @@ class FlatGradBucket:
             if p.grad is None or p.grad.data_ptr() != self.views[n].data_ptr():
                 p.grad = self.views[n]
 
-    def note_backward(self, flagged: bool) -> None:
-        """Called by the rasterizer's backward after it wrote into sink(): `flagged` = it set the flag of every row it
-        wrote.  The flags stay valid only while every such backward since the last zero_() was flagged."""
-        self.flags_valid = flagged and self.sparse_ok and (self.flags_valid or self._clean)
+    def note_backward(self) -> None:
+        """Called by the rasterizer's backward after it wrote into sink(); it flags every row it writes.  The flags
+        become valid with the first such backward after a zero_() and stay valid through the next ones."""
+        self.flags_valid = self.sparse_ok and (self.flags_valid or self._clean)
         self._clean = False
 
     def sink(self) -> Dict[str, Tensor]:

@@ -174,10 +174,7 @@ class RasterSettings:
     exact_lists: bool = False  # parity mode: gsplat's full bbox intersection lists instead of the precise-hit lists
     sync_free: bool = False  # size the intersection buffers from past views instead of reading the count back
     fixed_capacity: int = 0  # > 0: use exactly this many intersection slots, no host bookkeeping (CUDA-graph capture)
-    compact_bwd: bool = False  # project_bwd walks the depth-sorted index (validated in round 2: slower; kept for A/B)
     list_shift: int = 2  # intersection lists per (16 << list_shift)-pixel supertile; forced to 0 by exact_lists
-    touched_bwd: bool = True  # project_bwd only over the Gaussians that received a raster gradient
-    variant: int = 0  # kernel tuning knob (csrc/raster.cu): bit 0 butterfly reduction in the backward
 
 
 class RasterOutput(NamedTuple):
@@ -234,7 +231,6 @@ def _base_args(s: RasterSettings, n: int, sh_bases: int, accumulate: bool = Fals
         flags |= L.FLAG_EXACT_LISTS
     a.flags = flags
     a.list_shift = 0 if s.exact_lists else int(s.list_shift)
-    a.variant = int(s.variant)
     a.near_plane, a.far_plane, a.eps2d, a.radius_clip = s.near_plane, s.far_plane, s.eps2d, 0.0
     a.background[0], a.background[1], a.background[2] = s.background
     return a
@@ -372,7 +368,6 @@ class _DnRasterize(torch.autograd.Function):
 
         ctx.settings, ctx.n, ctx.sh_bases, ctx.n_isects, ctx.host_cam = s, n, sh_bases, n_isects, host_cam
         ctx.save_for_backward(means, quats, scales, opac, sh_dc, sh_rest, viewmat, K, c2w if s.render_normals else None)
-        ctx.ws_scan = ws_scan if s.compact_bwd else None
         ctx.state = dict(radii=radii, records=records, flatten_ids=flatten_ids, tile_offsets=tile_offsets,
                          out_rgb=out_rgb, out_depth=out_depth, out_alpha=out_alpha, out_normal=out_normal, last_ids=last_ids,
                          normal_norm=normal_norm, clamp_mask=clamp_mask, means2d=means2d)
@@ -420,13 +415,12 @@ class _DnRasterize(torch.autograd.Function):
         v_normal = prep(v_normal) if s.render_normals else None
         sink = ctx.grad_sink
         touched = grad_records = None
-        if s.touched_bwd and not s.compact_bwd:
-            if sink is not None:
-                # the caller's buffers: a FlatGradBucket keeps the flags across backwards and grad_records always zero
-                # (DNR_FLAG_PERSISTENT_WS); parallel.PeerGradBucket's peers read its flags over NVLink
-                touched, grad_records = sink.get("touched"), sink.get("grad_records")
-            if touched is None:
-                touched, grad_records = torch.empty(n, dtype=torch.uint8, device=dev), None
+        if sink is not None:
+            # the caller's buffers: a FlatGradBucket keeps the flags across backwards and grad_records always zero
+            # (DNR_FLAG_PERSISTENT_WS); parallel.PeerGradBucket's peers read its flags over NVLink
+            touched, grad_records = sink.get("touched"), sink.get("grad_records")
+        if touched is None:
+            touched, grad_records = torch.empty(n, dtype=torch.uint8, device=dev), None
         persistent = grad_records is not None
         if grad_records is None:
             grad_records = torch.empty(n, L.GRAD_FLOATS, **f32)
@@ -446,29 +440,21 @@ class _DnRasterize(torch.autograd.Function):
             a.flags |= L.FLAG_PERSISTENT_WS
         L.check(_timed("raster_bwd", lib.dnr_raster_bwd, C.byref(a), st), "dnr_raster_bwd")
         del keep
-        if s.compact_bwd:
-            a.flags |= L.FLAG_COMPACT_BWD
-            a.depth_order = lib.dnr_depth_order_ptr(ctx.ws_scan.data_ptr(), n)
-        scattered = s.compact_bwd or touched is not None  # accumulate-only kernels: buffers must be pre-zeroed
-        if touched is not None:
-            a.flags |= L.FLAG_TOUCHED_BWD
+        # project_bwd visits only the flagged Gaussians and accumulates: every gradient buffer starts at zero
+        a.flags |= L.FLAG_ACCUMULATE
         if sink is not None:
             # write straight into the caller's (pre-zeroed, e.g. flat all-reduce bucket) gradient buffers
-            a.flags |= L.FLAG_ACCUMULATE
             v_means, v_quats, v_scales = sink["means"], sink["quats"], sink["scales"]
             v_opac, v_sh_dc, v_sh_rest = sink["opacities"], sink["features_dc"], sink["features_rest"]
         else:
-            alloc = torch.zeros_like if scattered else torch.empty_like
-            if scattered:
-                a.flags |= L.FLAG_ACCUMULATE
-            v_means = alloc(means)
-            v_quats = alloc(quats)
-            v_scales = alloc(scales)
-            v_opac = alloc(opac)
-            v_sh_dc = alloc(sh_dc)
-            v_sh_rest = alloc(sh_rest)
-        v_m2d = (torch.zeros if touched is not None else torch.empty)(n, 2, **f32)
-        v_m2d_abs = (torch.zeros if touched is not None else torch.empty)(n, 2, **f32)
+            v_means = torch.zeros_like(means)
+            v_quats = torch.zeros_like(quats)
+            v_scales = torch.zeros_like(scales)
+            v_opac = torch.zeros_like(opac)
+            v_sh_dc = torch.zeros_like(sh_dc)
+            v_sh_rest = torch.zeros_like(sh_rest)
+        v_m2d = torch.zeros(n, 2, **f32)
+        v_m2d_abs = torch.zeros(n, 2, **f32)
         # camera optimisation: d(loss)/d(viewmat) only when the viewmat asks for it (otherwise the launch is unchanged)
         v_viewmat = torch.zeros(4, 4, **f32) if ctx.needs_input_grad[6] else None
         _set(a, v_means=v_means, v_quats=v_quats, v_scales=v_scales, v_opacities=v_opac, v_sh_dc=v_sh_dc,
@@ -483,7 +469,7 @@ class _DnRasterize(torch.autograd.Function):
             v_viewmat = v_viewmat.to(vdev).view(shape)
         if sink is not None:
             if sink.get("bucket") is not None:
-                sink["bucket"].note_backward(persistent)
+                sink["bucket"].note_backward()
             return (None,) * 6 + (v_viewmat,) + (None,) * 4
         return (v_means, v_quats, v_scales, v_opac.view(ctx.opac_shape), v_sh_dc, v_sh_rest, v_viewmat, None, None, None,
                 None)
@@ -556,8 +542,8 @@ def dn_rasterize(
     far_plane: float = 1e10, eps2d: float = 0.3, antialiased: bool = False,
     background: Sequence[float] = (0.0, 0.0, 0.0), render_normals: bool = True, c2w: Optional[Tensor] = None,
     activated: bool = False, surface_normal: bool = True, grad_sink: Optional[dict] = None,
-    exact_lists: bool = False, sync_free: bool = False, fixed_capacity: int = 0, compact_bwd: bool = False,
-    list_shift: int = 2, touched_bwd: bool = True, variant: int = 0, stats: Optional[Tensor] = None,
+    exact_lists: bool = False, sync_free: bool = False, fixed_capacity: int = 0, list_shift: int = 2,
+    stats: Optional[Tensor] = None,
 ) -> RasterOutput:
     """Renders one view.  Inputs are the reference's RAW gauss_params (log-scales, opacity logits,
     un-normalised wxyz quats, SH coefficients split as features_dc / features_rest) unless
@@ -569,8 +555,7 @@ def dn_rasterize(
     settings = RasterSettings(width=int(width), height=int(height), sh_degree=int(sh_degree), near_plane=near_plane,
                               far_plane=far_plane, eps2d=eps2d, antialiased=antialiased, render_normals=render_normals,
                               activated=activated, background=bg, surface_normal=surface_normal, exact_lists=exact_lists,
-                              sync_free=sync_free, fixed_capacity=int(fixed_capacity), compact_bwd=compact_bwd,
-                              list_shift=int(list_shift), touched_bwd=touched_bwd, variant=int(variant))
+                              sync_free=sync_free, fixed_capacity=int(fixed_capacity), list_shift=int(list_shift))
     info: dict = {}
     if stats is not None:
         info["stats"] = stats

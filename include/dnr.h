@@ -48,16 +48,14 @@ extern "C" {
 #define DNR_FLAG_ACTIVATED 1u   /* scales/opacities are already exp()/sigmoid()-activated (gsplat's signature) */
 #define DNR_FLAG_ANTIALIASED 2u /* rasterize_mode == "antialiased": opacity *= compensation */
 #define DNR_FLAG_NORMALS 4u     /* predict_normals: render the per-Gaussian normal channels */
-#define DNR_FLAG_ACCUMULATE 8u  /* project_bwd adds into the parameter-gradient buffers */
-#define DNR_FLAG_COMPACT_BWD 64u /* project_bwd walks the depth-sorted index (validated, but slower than DNR_FLAG_TOUCHED_BWD: kept for A/B)
-                                    (a->depth_order), so only visible Gaussians occupy lanes; needs DNR_FLAG_ACCUMULATE */
+#define DNR_FLAG_ACCUMULATE 8u  /* project_bwd adds into the parameter-gradient buffers (required by dnr_project_bwd) */
 #define DNR_FLAG_HOST_CAMERA 32u /* camera passed by value in host_cam[] (no device reads, no H2D copy) */
 #define DNR_FLAG_EXACT_LISTS 16u /* parity mode: emit gsplat's full bbox intersection lists (no precise-hit cull) */
-#define DNR_FLAG_TOUCHED_BWD 128u /* project_bwd processes only Gaussians with touched[g] != 0 (needs DNR_FLAG_ACCUMULATE) */
+/* 64u and 128u are retired (they selected project_bwd kernels that no longer exist) and are not to be reused */
 #define DNR_FLAG_PERSISTENT_WS 256u /* raster_bwd: touched and grad_records are the caller's persistent buffers and are not
-                                       cleared.  grad_records must be all zero on entry (the DNR_FLAG_TOUCHED_BWD project_bwd
-                                       that follows leaves it so); the flags accumulate over calls until the caller clears
-                                       them (dnr_grad_zero) */
+                                       cleared.  grad_records must be all zero on entry (the project_bwd that follows
+                                       leaves it so); the flags accumulate over calls until the caller clears them
+                                       (dnr_grad_zero) */
 
 /* floats per packed per-Gaussian raster record, without / with normals */
 #define DNR_REC_FLOATS 12
@@ -133,8 +131,8 @@ typedef struct DnrArgs {
   const float* v_depth;  /* [H,W]   or NULL */
   const float* v_normal; /* [H,W,3] or NULL */
   const float* v_alpha;  /* [H,W]   or NULL */
-  float* grad_records;   /* [N, DNR_GRAD_FLOATS] zeroed by dnr_raster_bwd (unless DNR_FLAG_PERSISTENT_WS); the
-                            DNR_FLAG_TOUCHED_BWD project_bwd writes zeros back to every row it consumes */
+  float* grad_records;   /* [N, DNR_GRAD_FLOATS] zeroed by dnr_raster_bwd (unless DNR_FLAG_PERSISTENT_WS);
+                            dnr_project_bwd writes zeros back to every row it consumes */
 
   /* ---- projection backward outputs ---- */
   float* v_means;       /* [N,3] */
@@ -157,7 +155,7 @@ typedef struct DnrArgs {
   int32_t use_normal_loss;
   /* with DNR_FLAG_HOST_CAMERA: [0..15] viewmat, [16..19] fx fy cx cy, [20..31] c2w[3,4]; viewmat/K/c2w pointers unused */
   float host_cam[32];
-  const int32_t* depth_order; /* [N] Gaussian ids sorted by depth, visible first (dnr_depth_order_ptr); COMPACT_BWD only */
+  const void* reserved2; /* unused; keeps the layout (and so the kernels' parameter offsets) stable */
 
   /* ---- loss gradients evaluated inside dnr_raster_bwd (BASELINE north_star: regularisers fused into the backward) ----
    * With DNR_LOSS_FUSED_BWD the per-pixel gradients of
@@ -167,16 +165,17 @@ typedef struct DnrArgs {
    * are computed in the kernel's prologue from the rendered maps instead of being read from v_rgb / v_depth / v_normal
    * images; non-NULL v_rgb / v_depth / v_normal / v_alpha are ADDED (e.g. the SSIM gradient). */
   uint32_t loss_flags;   /* DNR_LOSS_* */
-  int32_t variant;       /* kernel tuning knob (0 = default); see csrc/raster.cu */
+  int32_t reserved3;     /* unused, as reserved2 */
   const void* gt_image;  /* [H,W,3] photometric target: uint8 (DNR_LOSS_IMG_U8, scaled by 1/255) or fp32 */
   const float* v_l1;     /* [1] device scalar */
-  uint8_t* touched;      /* [N] or NULL: dnr_raster_bwd sets touched[g] = 1 for every Gaussian that received a gradient
-                            (zeroed by the call unless DNR_FLAG_PERSISTENT_WS); dnr_project_bwd then skips the others
-                            (DNR_FLAG_TOUCHED_BWD) */
+  uint8_t* touched;      /* [N]: dnr_raster_bwd sets touched[g] = 1 for every Gaussian that received a gradient
+                            (zeroed by the call unless DNR_FLAG_PERSISTENT_WS); dnr_project_bwd processes only the
+                            flagged Gaussians.  Required by dnr_project_bwd; dnr_raster_bwd alone accepts NULL (without
+                            DNR_FLAG_PERSISTENT_WS) */
   uint64_t* stats; /* [4] or NULL: += {list entries walked, entries kept by the tile filter} (fwd: [0],[1]; bwd: [2],[3]) */
   float* v_viewmat; /* [4,4] or NULL: dnr_project_bwd ADDS d(loss)/d(viewmat) (camera optimisation; the caller zeroes it
-                       first; row 3 is left alone).  Works with DNR_FLAG_HOST_CAMERA too; not with DNR_FLAG_COMPACT_BWD
-                       (DNR_E_OPTION).  The normals' c2w is treated as a separate constant. */
+                       first; row 3 is left alone).  Works with DNR_FLAG_HOST_CAMERA too.  The normals' c2w is treated
+                       as a separate constant. */
 } DnrArgs;
 
 /* loss_flags */
@@ -198,8 +197,6 @@ size_t dnr_bin_scan_workspace_bytes(int32_t n_gauss);
  * pass NULL to stay asynchronous and size by capacity. */
 int dnr_bin_scan(const DnrArgs* a, void* stream, int64_t* n_isects_host);
 size_t dnr_bin_sort_workspace_bytes(int32_t n_gauss, int64_t n_isects, int32_t n_tiles);
-/* Device pointer to the depth-sorted Gaussian ids inside a bin_scan workspace (valid after dnr_bin_scan). */
-const int32_t* dnr_depth_order_ptr(void* ws_scan, int32_t n_gauss);
 int dnr_bin_sort(const DnrArgs* a, void* stream);
 
 int dnr_raster_fwd(const DnrArgs* a, void* stream);

@@ -6,7 +6,6 @@ default.
 Rows (one JSON line each):
   ssim        FusedSSIM fwd+bwd  vs  dn_model.ssim (torch convs + autograd) at 1920x1080x3
   adam        FusedAdam (1 launch) vs  7 x torch.optim.Adam (default foreach) and fused=True, N Gaussians, SH degree 3
-  project_bwd default vs DNR_FLAG_COMPACT_BWD on the bench scene (stage events)
   camera_opt  project_bwd with vs without the view-matrix gradient (stage events), and the captured 1080p training step
               (GraphedTrainStep + FusedAdam) with camera optimisation off vs SO3xR3
   mesh        TSDF fusion of 200 ring views at 1920x1080 into a 512^3 grid over the scene cube (render + integrate, and
@@ -109,34 +108,6 @@ def bench_adam():
           "torch_foreach_ms": timed(lambda: [o.step() for o in ref], args.reps),
           "torch_fused_ms": timed(lambda: [o.step() for o in ref_fused], args.reps),
           "fused_GBps": floats * 28 / t_f / 1e6, "param_abs_err_after_1_step": err})
-
-
-def bench_project_bwd():
-    import dn_splatter_b200.rasterize as R
-    from dn_splatter_b200 import dn_rasterize, get_viewmat
-    from dn_splatter_b200.synthetic import BACKGROUND, make_scene, ring_cameras
-
-    W, H = 1920, 1080
-    cam = ring_cameras(8, W, H)[3]
-    K = torch.tensor([[cam["fx"], 0, cam["cx"]], [0, cam["fy"], cam["cy"]], [0, 0, 1]], dtype=torch.float32)
-    vm = get_viewmat(cam["c2w"])
-    res = {}
-    grads = {}
-    for compact in (False, True):
-        p = {k: v.cuda().requires_grad_(True) for k, v in make_scene(args.n, seed=0).items()}
-        out = dn_rasterize(p["means"], p["quats"], p["scales"], p["opacities"], p["features_dc"], p["features_rest"], vm, K, W, H,
-                           background=BACKGROUND, c2w=cam["c2w"], compact_bwd=compact)
-        loss = (out.rgb.sum() + out.depth.sum() * 0.1 + out.normal.sum()) * 1e-3
-        R.STAGE_EVENTS = []
-        for _ in range(args.reps):
-            gr = torch.autograd.grad(loss, list(p.values()), retain_graph=True)
-        torch.cuda.synchronize()
-        t = sorted(a.elapsed_time(b) for name, a, b in R.STAGE_EVENTS if name == "project_bwd")
-        R.STAGE_EVENTS = None
-        res[compact] = t[len(t) // 2]
-        grads[compact] = gr
-    rel = max(float((x - y).norm() / (x.norm() + 1e-30)) for x, y in zip(grads[False], grads[True]))
-    emit({"row": "project_bwd", "default_ms": res[False], "compact_ms": res[True], "grad_rel_err": rel})
 
 
 def bench_camera_opt():
@@ -520,8 +491,7 @@ def bench_mesh_eval():
     emit(row)
 
 
-for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("project_bwd", bench_project_bwd),
-                 ("camera_opt", bench_camera_opt), ("knn", bench_knn),
+for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("camera_opt", bench_camera_opt), ("knn", bench_knn),
                  ("render_service", bench_render_service), ("mesh", bench_mesh), ("poisson", bench_poisson),
                  ("mesh_eval", bench_mesh_eval)):
     if args.only and name not in args.only.split(","):

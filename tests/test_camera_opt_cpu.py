@@ -265,7 +265,7 @@ def test_two_rank_trainer_keeps_poses_identical_and_equal_to_one_process_over_th
     torch.testing.assert_close(torch.from_numpy(got), want, rtol=1e-4, atol=1e-7)
 
 
-def test_project_bwd_rejects_viewmat_gradient_on_the_compact_path():
+def test_project_bwd_requires_touched_flags_and_accumulation():
     import ctypes as C
 
     from dn_splatter_b200 import _lib as L
@@ -274,9 +274,9 @@ def test_project_bwd_rejects_viewmat_gradient_on_the_compact_path():
     a = L.DnrArgs()
     a.n_gauss, a.width, a.height, a.tile_size, a.sh_degree, a.sh_bases = 10, 32, 32, 16, 0, 1
     for name in ("viewmat", "K", "means", "quats", "scales", "opacities", "sh_dc", "radii", "grad_records", "v_means",
-                 "v_quats", "v_scales", "v_opacities", "v_sh_dc"):
-        setattr(a, name, 16)  # non-NULL dummies: the option checks come first, nothing is dereferenced
-    a.flags = L.FLAG_COMPACT_BWD | L.FLAG_ACCUMULATE
-    assert lib.dnr_project_bwd(C.byref(a), None) == -1  # no depth_order: the compact path's own NULL check
-    a.v_viewmat = 16
-    assert lib.dnr_project_bwd(C.byref(a), None) == -3  # DNR_E_OPTION: the compact path has no viewmat gradient
+                 "v_quats", "v_scales", "v_opacities", "v_sh_dc", "v_viewmat"):
+        setattr(a, name, 16)  # non-NULL dummies: the argument checks come first, nothing is dereferenced
+    a.flags = L.FLAG_ACCUMULATE
+    assert lib.dnr_project_bwd(C.byref(a), None) == -1  # DNR_E_NULL: no touched flags
+    a.touched, a.flags = 16, 0
+    assert lib.dnr_project_bwd(C.byref(a), None) == -3  # DNR_E_OPTION: the kernel only accumulates

@@ -70,19 +70,20 @@ def _raw_cases():
     out = []
     for mode in ("classic", "antialiased"):
         for sh in (0, 3):
-            for touched in (True, False):
+            for cam_on in ("device", "host"):
                 for route in ("rgb", "depth", "normal", "alpha", "all"):
                     if mode == "antialiased" and route == "normal":
                         continue  # one antialiased pass composites normals with the compensated opacity (see below)
-                    out.append((mode, sh, touched, route))
+                    out.append((mode, sh, cam_on, route))
     return out
 
 
 @needs_cuda
-@pytest.mark.parametrize("mode,sh,touched,route", _raw_cases(),
-                         ids=[f"{m}-sh{s}-{'touched' if t else 'dense'}-{r}" for m, s, t, r in _raw_cases()])
-def test_viewmat_gradient_matches_fp64_oracle(mode, sh, touched, route):
-    """Raw d(loss)/d(viewmat) at a ragged 81x49 frame.  The single-pass antialiased render composites the normal image
+@pytest.mark.parametrize("mode,sh,cam_on,route", _raw_cases(),
+                         ids=[f"{m}-sh{s}-{c}cam-{r}" for m, s, c, r in _raw_cases()])
+def test_viewmat_gradient_matches_fp64_oracle(mode, sh, cam_on, route):
+    """Raw d(loss)/d(viewmat) at a ragged 81x49 frame, with the viewmat on the device or on the host (then the camera
+    reaches the kernels by value: DNR_FLAG_HOST_CAMERA).  The single-pass antialiased render composites the normal image
     with the compensated opacity while the reference's normal pass uses the plain one, so its normal route is left out
     (the model's two-pass mode is covered end to end below)."""
     from dn_splatter_b200 import dn_rasterize
@@ -102,11 +103,11 @@ def test_viewmat_gradient_matches_fp64_oracle(mode, sh, touched, route):
     p = {k: v.cuda().requires_grad_(True) for k, v in params.items()}
     c2w = cam["c2w"].cuda()
     K = torch.tensor([[cam["fx"], 0, cam["cx"]], [0, cam["fy"], cam["cy"]], [0, 0, 1]], dtype=torch.float32, device="cuda")
-    vm = orc.vm.detach().float().cuda().requires_grad_(True)
+    vm = orc.vm.detach().float().to("cuda" if cam_on == "device" else "cpu").requires_grad_(True)
     out = dn_rasterize(p["means"], p["quats"], p["scales"], p["opacities"], p["features_dc"], p["features_rest"], vm, K, W,
-                       H, sh_degree=sh, background=BACKGROUND, c2w=c2w, antialiased=mode == "antialiased",
-                       touched_bwd=touched)
+                       H, sh_degree=sh, background=BACKGROUND, c2w=c2w, antialiased=mode == "antialiased")
     route_loss(out.rgb, out.depth, out.normal, out.alpha, route, mask, use_normal=use_normal).backward()
+    assert vm.grad.device == vm.device
     got = vm.grad.cpu()
     assert not bool(got[3].any()), "row 3 of the viewmat gets no gradient"
     err = rel_err(got[:3], want[:3])
@@ -118,7 +119,7 @@ def test_viewmat_gradient_matches_fp64_oracle(mode, sh, touched, route):
         v.grad = None
     out = dn_rasterize(p["means"], p["quats"], p["scales"], p["opacities"], p["features_dc"], p["features_rest"],
                        vm.detach(), K, W, H, sh_degree=sh, background=BACKGROUND, c2w=c2w,
-                       antialiased=mode == "antialiased", touched_bwd=touched)
+                       antialiased=mode == "antialiased")
     route_loss(out.rgb, out.depth, out.normal, out.alpha, route, mask, use_normal=use_normal).backward()
     for k in p:
         assert rel_err(p[k].grad, g1[k]) <= 1e-5, k

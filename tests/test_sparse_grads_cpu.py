@@ -17,21 +17,19 @@ def _bucket(n=50):
     return FlatGradBucket({k: torch.nn.Parameter(torch.zeros(*s)) for k, s in shapes.items()})
 
 
-def test_flags_are_valid_only_after_flagged_backwards_since_a_zero():
+def test_flags_are_valid_only_after_backwards_since_a_zero():
     b = _bucket()
     assert not b.flags_valid  # a fresh bucket may be filled by other means (flat.copy_)
-    b.note_backward(True)
+    b.note_backward()
     assert not b.flags_valid  # ... so a backward without a zero_() first does not validate it
     b.zero_()  # dense while the flags are not valid (no kernel: runs on the CPU)
-    b.note_backward(True)
-    b.note_backward(True)  # the antialiased + normals model: two flagged passes per step
+    b.note_backward()
+    b.note_backward()  # the antialiased + normals model: two flagged passes per step
     assert b.flags_valid
-    b.note_backward(False)  # an unflagged pass (touched_bwd=False / compact_bwd) wrote rows the flags miss
-    b.note_backward(True)
-    assert not b.flags_valid
+    b = _bucket()
     b.zero_()
     b.sparse_ok = False  # parameter-only loss terms besides min-scale (dn_model.enable_flat_grads)
-    b.note_backward(True)
+    b.note_backward()
     assert not b.flags_valid
     assert b.dense_params == {"scales"} and b.n_gauss == 50
     assert b.grad_records.shape == (50, L.GRAD_FLOATS) and b.touched.dtype == torch.uint8
