@@ -221,12 +221,14 @@ __global__ void __launch_bounds__(256) scale_loss_bwd_kernel(const float* __rest
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
   if (i >= n) return;
   const float vl = v_loss ? __ldg(v_loss) : 1.0f;
-  const float s0 = scales[i * 3], s1 = scales[i * 3 + 1], s2 = scales[i * 3 + 2];
+  // torch.exp(scales).min(1) picks the FIRST index of the smallest exp: distinct log-scales whose exp rounds to one fp32
+  // value are a tie there, so the argmin is taken over the exps, not over the log-scales
+  const float e0 = expf(scales[i * 3]), e1 = expf(scales[i * 3 + 1]), e2 = expf(scales[i * 3 + 2]);
   int idx = 0;
-  float m = s0;
-  if (s1 < m) { m = s1; idx = 1; }
-  if (s2 < m) { m = s2; idx = 2; }
-  const float g = vl * expf(m) / (float)n;
+  float m = e0;
+  if (e1 < m) { m = e1; idx = 1; }
+  if (e2 < m) { m = e2; idx = 2; }
+  const float g = vl * m / (float)n;
   v_scales[i * 3 + 0] = idx == 0 ? g : 0.f;
   v_scales[i * 3 + 1] = idx == 1 ? g : 0.f;
   v_scales[i * 3 + 2] = idx == 2 ? g : 0.f;

@@ -296,7 +296,8 @@ __device__ __forceinline__ void fused_loss_grads(const DnrArgs& a, int i, int j,
     float w = 1.0f / __ldg(a.loss_partials + 1);
     if (a.depth_loss_type == 1) {
       const float wx = edge_weight(a, p, pr), wy = edge_weight(a, p, pd);  // exp(0) = 1 at the clamped border: masked below
-      w = (j < W - 1 ? wx : 0.f) / __ldg(a.loss_partials + 1) + (i < H - 1 ? wy : 0.f) / __ldg(a.loss_partials + 3);
+      // select, not multiply: a count is 0 when no valid pixel has that neighbour, and 0 / 0 would poison the pixel
+      w = (j < W - 1 ? wx / __ldg(a.loss_partials + 1) : 0.f) + (i < H - 1 ? wy / __ldg(a.loss_partials + 3) : 0.f);
     }
     const float e = od - gd;
     float dval;

@@ -306,6 +306,7 @@ class DNSplatterModel(_ModelBase):
             self.tv_loss = TVLoss()
         if cfg.regularization_strategy == "dn-splatter":
             self.regularization_strategy = DNRegularization()
+            self.regularization_strategy.fuse_backward = cfg.fuse_loss_backward
         elif cfg.regularization_strategy == "ags-mesh":
             self.regularization_strategy = AGSMeshRegularization()
         else:

@@ -335,7 +335,8 @@ class DNRegularization(RegularizationStrategy):
         return (not with_depth) or self.depth_loss_type in _FUSED_DEPTH
 
     fuse_backward = True
-    """Hand the backward of the fused terms to dnr_raster_bwd when the maps are direct raster outputs."""
+    """Hand the backward of the fused terms to dnr_raster_bwd when the maps are direct raster outputs; DNSplatterModel sets
+    it from DNSplatterModelConfig.fuse_loss_backward (False: dnr_loss_bwd writes gradient images)."""
 
     def get_loss(self, pred_depth, gt_depth, pred_normal, gt_normal, **kwargs):
         with_depth = self.depth_loss is not None

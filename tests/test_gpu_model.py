@@ -378,13 +378,18 @@ def test_fused_adam_matches_torch_adam():
 @needs_cuda
 @pytest.mark.parametrize("depth_type,ssim_lambda", [("EdgeAwareLogL1", 0.0), ("EdgeAwareLogL1", 0.2), ("LogL1", 0.0),
                                                      ("L1", 0.2), ("mse", 0.0)])
-def test_loss_gradients_fused_into_raster_bwd_match_the_gradient_image_path(depth_type, ssim_lambda):
+def test_loss_gradients_fused_into_raster_bwd_match_the_gradient_image_path(depth_type, ssim_lambda, monkeypatch):
     """BASELINE north_star: the Depth / Normal / TV regularisers (and the photometric L1) are differentiated inside
     dnr_raster_bwd.  The same step with the losses' own backward kernels writing gradient images (fuse_loss_backward =
-    False) and with host-resident float maps (the generic torch path of get_loss_dict) must give the same loss and the
-    same parameter gradients."""
+    False: dnr_loss_bwd runs, and only there) and with host-resident float maps (the generic torch path of get_loss_dict)
+    must give the same loss and the same parameter gradients."""
+    from dn_splatter_b200 import _lib as L
     from dn_splatter_b200.losses import DepthLossType
 
+    lib = L.load()
+    loss_bwd_calls = []
+    orig = lib.dnr_loss_bwd
+    monkeypatch.setitem(lib.__dict__, "dnr_loss_bwd", lambda *args: loss_bwd_calls.append(1) or orig(*args))
     params, cam = scene_and_camera(1200, 144, 112, view=2)
     H, W = 112, 144
     g = torch.Generator().manual_seed(11)
@@ -399,7 +404,9 @@ def test_loss_gradients_fused_into_raster_bwd_match_the_gradient_image_path(dept
         batch = {k: v.to(dev) for k, v in raw.items()}
         out = m.get_outputs(_camera(cam))
         ld = m.get_loss_dict(out, batch)
+        loss_bwd_calls.clear()
         (ld["main_loss"] + ld["scale_reg"]).backward()
+        assert len(loss_bwd_calls) == (1 if name == "images" else 0), (name, len(loss_bwd_calls))
         runs[name] = (float(ld["main_loss"]), {k: m.gauss_params[k].grad.clone() for k in
                                                 ("means", "quats", "scales", "opacities", "features_dc", "features_rest")},
                       m.xys_flat.absgrad.clone())
