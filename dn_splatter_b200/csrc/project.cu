@@ -237,6 +237,16 @@ __device__ __forceinline__ int argmin3(float s0, float s1, float s2) {
   return idx;
 }
 
+// Sign of the per-Gaussian normal: -1 when the unit normal n faces away from the camera (its dot product with the
+// normalised view vector vd = campos - mean is negative).  The forward and the backward both take it from here: for a
+// Gaussian seen edge-on the dot product is ~0, and a differently rounded expression in the backward would differentiate
+// the normal with the opposite sign from the one that was rendered.
+__device__ __forceinline__ float normal_sign(const float n[3], const float vd[3]) {
+  const float vn = sqrtf((vd[0] * vd[0] + vd[1] * vd[1]) + vd[2] * vd[2]);
+  const float d = (n[0] * (vd[0] / vn) + n[1] * (vd[1] / vn)) + n[2] * (vd[2] / vn);
+  return d < 0.f ? -1.0f : 1.0f;
+}
+
 template <bool NORMALS>
 __global__ void __launch_bounds__(256) project_fwd_kernel(const DnrArgs a) {
   const int i = blockIdx.x * blockDim.x + threadIdx.x;
@@ -262,9 +272,7 @@ __global__ void __launch_bounds__(256) project_fwd_kernel(const DnrArgs a) {
       n[k] = n[k] / nn;
       vd[k] = cam.c2wT[k] - a.means[i * 3 + k];
     }
-    const float vn = sqrtf((vd[0] * vd[0] + vd[1] * vd[1]) + vd[2] * vd[2]);
-    const float d = (n[0] * (vd[0] / vn) + n[1] * (vd[1] / vn)) + n[2] * (vd[2] / vn);
-    const float sgn = d < 0.f ? -1.0f : 1.0f;
+    const float sgn = normal_sign(n, vd);
 #pragma unroll
     for (int k = 0; k < 3; ++k) nw[k] = sgn * n[k];
 #pragma unroll
@@ -490,8 +498,7 @@ __device__ __forceinline__ void project_bwd_gauss(const DnrArgs& a, int i, int n
     float vd[3], nu[3];
 #pragma unroll
     for (int k = 0; k < 3; ++k) { nu[k] = n[k] / nn; vd[k] = cam.c2wT[k] - a.means[i * 3 + k]; }
-    const float d = nu[0] * vd[0] + nu[1] * vd[1] + nu[2] * vd[2];
-    const float sgn = d < 0.f ? -1.0f : 1.0f;
+    const float sgn = normal_sign(nu, vd);
     float vnw[3];
 #pragma unroll
     for (int r = 0; r < 3; ++r)
