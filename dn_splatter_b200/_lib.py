@@ -119,6 +119,7 @@ KERNELS_PER_CALL = {
     "dnr_knn_build": (2, 1), "dnr_knn_query": (1, 0), "dnr_density": (1, 0), "dnr_ray_densities": (1, 0),
     "dnr_tsdf_integrate": (1, 0), "dnr_mc_count": (1, 6), "dnr_mc_emit": (2, 0),
     "dnr_grid_sample": (1, 0), "dnr_mesh_visibility": (1, 0),
+    "dnr_rgb_metrics": (1, 0), "dnr_depth_metrics": (1, 0), "dnr_normal_metrics": (8, 0),
 }
 LAUNCHES = {"handwritten": 0, "cub": 0}
 DEBUG_CAPTURE = os.environ.get("DNR_DEBUG_CAPTURE") == "1"
@@ -263,6 +264,16 @@ def load():
     lib.dnr_mesh_visibility.restype = C.c_int
     lib.dnr_mesh_visibility.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32,
                                         C.c_float, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_rgb_metrics.restype = C.c_int
+    lib.dnr_rgb_metrics.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p,
+                                    C.c_void_p]
+    lib.dnr_depth_metrics.restype = C.c_int
+    lib.dnr_depth_metrics.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_float, C.c_void_p, C.c_void_p]
+    lib.dnr_normal_metrics_workspace_bytes.restype = C.c_int64
+    lib.dnr_normal_metrics_workspace_bytes.argtypes = [C.c_int32, C.c_int32, C.c_int32]
+    lib.dnr_normal_metrics.restype = C.c_int
+    lib.dnr_normal_metrics.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_int64,
+                                       C.c_void_p, C.c_void_p]
     lib.dnr_ssim_bwd.restype = C.c_int
     lib.dnr_ssim_bwd.argtypes = [C.c_void_p, C.c_void_p, C.c_int32, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p,
                                  C.c_void_p]
@@ -282,7 +293,8 @@ EXPORTS = (
     "dnr_density", "dnr_ray_densities", "dnr_tsdf_integrate", "dnr_mc_count_workspace_bytes", "dnr_mc_count",
     "dnr_mc_emit_workspace_bytes", "dnr_mc_emit", "dnr_poisson_splat_workspace_bytes", "dnr_poisson_splat",
     "dnr_poisson_solve_workspace_bytes", "dnr_poisson_solve", "dnr_grid_sample", "dnr_mesh_depth_workspace_bytes",
-    "dnr_mesh_depth", "dnr_mesh_visibility",
+    "dnr_mesh_depth", "dnr_mesh_visibility", "dnr_rgb_metrics", "dnr_depth_metrics", "dnr_normal_metrics_workspace_bytes",
+    "dnr_normal_metrics",
 )
 
 

@@ -29,6 +29,12 @@ __constant__ float c_win[11] = {1.028380357e-03f, 7.598758209e-03f, 3.600077331e
                                 2.660117149e-01f, 2.130055279e-01f, 1.093606874e-01f, 3.600077331e-02f, 7.598758209e-03f,
                                 1.028380357e-03f};
 
+__device__ __forceinline__ double warp_sum_f64(double v) {
+#pragma unroll
+  for (int o = 16; o > 0; o >>= 1) v += __shfl_xor_sync(0xffffffffu, v, o);
+  return v;
+}
+
 template <bool U8>
 __device__ __forceinline__ float ld_gt(const void* img, size_t idx) {
   return U8 ? __fmul_rn((float)((const uint8_t*)img)[idx], 1.0f / 255.0f) : ((const float*)img)[idx];
@@ -92,7 +98,9 @@ __device__ __forceinline__ void vpass(float (*s_mid)[SS_C][SS_H][SS_T], int c, i
 // NC = channels this launch handles per CTA (compile time: the index arithmetic of the halo load and of the work-item
 // loops is mul-shift instead of runtime integer division, which cost a third of the round-2a kernel's instructions);
 // c0 = first channel.
-template <bool U8, bool L1, int NC>
+// METRIC (evaluation, no gradient): blockIdx.z is the image of a [B,H,W,C] batch, no dmaps are written, the second sum is
+// (x - y)^2 instead of |x - y|, and sum_out is double [B,2] that receives one fp64 atomic per CTA per quantity.
+template <bool U8, bool L1, int NC, bool METRIC = false>
 __global__ void __launch_bounds__(SS_NT) ssim_fwd_kernel(const float* __restrict__ x, const void* __restrict__ y, int H, int W,
                                                         int C, int c0, float* __restrict__ dmaps, float* __restrict__ sum_out) {
   __shared__ __align__(16) float s_in[2][SS_C][SS_H][SS_P];
@@ -102,6 +110,11 @@ __global__ void __launch_bounds__(SS_NT) ssim_fwd_kernel(const float* __restrict
   const int tid = threadIdx.x;
   constexpr int nc = NC;
   const int i0 = blockIdx.y * SS_T - SS_R, j0 = blockIdx.x * SS_T - SS_R;
+  if constexpr (METRIC) {
+    const size_t img = (size_t)blockIdx.z * H * W * C;
+    x += img;
+    y = U8 ? (const void*)((const uint8_t*)y + img) : (const void*)((const float*)y + img);
+  }
   // halo load: consecutive threads walk (column, channel) of one image row -> contiguous global addresses
   for (int e = tid; e < SS_H * SS_H * NC; e += SS_NT) {
     const int c = e % NC, q = (e / NC) % SS_H, r = e / (NC * SS_H);
@@ -145,11 +158,31 @@ __global__ void __launch_bounds__(SS_NT) ssim_fwd_kernel(const float* __restrict
       }
       if (i < H && j < W) {
         const size_t p = ((size_t)i * W + j) * C + c0 + c;
-        dmaps[p] = d_mu; dmaps[n + p] = d_xx; dmaps[2 * n + p] = d_xy;
-        if (L1) lsum += fabsf(s_in[0][c][4 * g + o + SS_R][col + SS_R] - s_in[1][c][4 * g + o + SS_R][col + SS_R]);
+        if constexpr (METRIC) {
+          const float d = s_in[0][c][4 * g + o + SS_R][col + SS_R] - s_in[1][c][4 * g + o + SS_R][col + SS_R];
+          lsum += d * d;
+        } else {
+          dmaps[p] = d_mu; dmaps[n + p] = d_xx; dmaps[2 * n + p] = d_xy;
+          if (L1) lsum += fabsf(s_in[0][c][4 * g + o + SS_R][col + SS_R] - s_in[1][c][4 * g + o + SS_R][col + SS_R]);
+        }
       }
       ssum += s;
     }
+  }
+  if constexpr (METRIC) {
+    __shared__ double red_d[2][SS_NT / 32];
+    const double ds = warp_sum_f64(ssum), dl = warp_sum_f64(lsum);
+    if ((tid & 31) == 0) { red_d[0][tid >> 5] = ds; red_d[1][tid >> 5] = dl; }
+    __syncthreads();
+    if (tid == 0) {
+      double t = 0.0, tl = 0.0;
+#pragma unroll
+      for (int w = 0; w < SS_NT / 32; ++w) { t += red_d[0][w]; tl += red_d[1][w]; }
+      double* out = reinterpret_cast<double*>(sum_out) + 2 * blockIdx.z;
+      if (t != 0.0) atomicAdd(out, t);
+      if (tl != 0.0) atomicAdd(out + 1, tl);
+    }
+    return;
   }
   ssum = warp_sum(ssum);
   if (L1) lsum = warp_sum(lsum);
@@ -242,6 +275,27 @@ static int launch_ssim_bwd(const float* pred, const void* gt, int gt_is_u8, int 
     if (gt_is_u8) { if (nc == 3) DNR_SSIM_BWD(true, 3); else if (nc == 2) DNR_SSIM_BWD(true, 2); else DNR_SSIM_BWD(true, 1); }
     else { if (nc == 3) DNR_SSIM_BWD(false, 3); else if (nc == 2) DNR_SSIM_BWD(false, 2); else DNR_SSIM_BWD(false, 1); }
 #undef DNR_SSIM_BWD
+    DNR_CHECK_LAUNCH();
+  }
+  return 0;
+}
+
+// pred: [B,H,W,C] fp32; gt: [B,H,W,C] fp32, or uint8 read as value / 255 when gt_is_u8 != 0.  out [B,2] double, zeroed by
+// the call: per image the SSIM sum over the (H-10)(W-10)C interior and the sum of squared errors over all H W C values.
+extern "C" int dnr_rgb_metrics(const float* pred, const void* gt, int32_t gt_is_u8, int32_t B, int32_t H, int32_t W, int32_t C,
+                               double* out, void* stream) {
+  if (!pred || !gt || !out) return DNR_E_NULL;
+  if (B <= 0 || B > 65535 || H <= 2 * SS_R || W <= 2 * SS_R || C <= 0) return DNR_E_SIZE;
+  cudaStream_t s = (cudaStream_t)stream;
+  DNR_CUDA(cudaMemsetAsync(out, 0, 2 * (size_t)B * sizeof(double), s));
+  const dim3 grid((W + SS_T - 1) / SS_T, (H + SS_T - 1) / SS_T, B);
+  float* o = reinterpret_cast<float*>(out);
+  for (int c0 = 0; c0 < C; c0 += SS_C) {
+    const int nc = C - c0 < SS_C ? C - c0 : SS_C;
+#define DNR_SSIM_MET(U8, NC) ssim_fwd_kernel<U8, false, NC, true><<<grid, SS_NT, 0, s>>>(pred, gt, H, W, C, c0, nullptr, o)
+    if (gt_is_u8) { if (nc == 3) DNR_SSIM_MET(true, 3); else if (nc == 2) DNR_SSIM_MET(true, 2); else DNR_SSIM_MET(true, 1); }
+    else { if (nc == 3) DNR_SSIM_MET(false, 3); else if (nc == 2) DNR_SSIM_MET(false, 2); else DNR_SSIM_MET(false, 1); }
+#undef DNR_SSIM_MET
     DNR_CHECK_LAUNCH();
   }
   return 0;

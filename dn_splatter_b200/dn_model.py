@@ -5,7 +5,8 @@
 The class works standalone (nerfstudio is optional): cameras are duck-typed (cameras.Cameras or
 nerfstudio's), parameters keep the reference's names so checkpoints stay interchangeable
 (gauss_params: means, scales, quats, features_dc, features_rest, opacities, normals).
-What is deliberately NOT here: densification (refinement_after), metrics/LPIPS, SuGaR density helpers,
+Evaluation (get_metrics_dict, get_image_metrics_and_images; reference :731-926) runs on the metric kernels of
+metrics.py; LPIPS only through a user-set `model.lpips` callable.  What is deliberately NOT here: SuGaR density helpers,
 crop boxes — outside the hot path (SURVEY.md §2.1 #1, §8f).  Camera optimisation (camera_opt.py) renders the
 training views with the optimised pose; the projection backward returns the pose gradient.
 """
@@ -22,6 +23,7 @@ from torch import Tensor
 from .camera_opt import compose as compose_pose
 from .cameras import Cameras, is_camera
 from .losses import DepthLoss, DepthLossType, TVLoss, ssim  # noqa: F401  (ssim re-exported)
+from .metrics import DepthMetrics, NormalMetrics, rgb_metrics, tf_resize, u8_as_float
 from .rasterize import dn_rasterize, get_viewmat, raster_holder, to_device_async
 from .regularization_strategy import (AGSMeshRegularization, DNRegularization, FusedL1, FusedPhotometric, FusedSSIM,
                                       u8_to_float)
@@ -275,6 +277,10 @@ class DNSplatterModel(_ModelBase):
         else:
             self.background_color = torch.tensor({"black": [0.0, 0.0, 0.0], "white": [1.0, 1.0, 1.0]}[cfg.background_color])
         self.mse_loss = torch.nn.MSELoss()
+        # LPIPS needs network weights: rgb_lpips is reported only when the user sets a callable lpips(gt, pred) here
+        self.lpips = None
+        self.depth_metrics = DepthMetrics()
+        self.normal_metrics = NormalMetrics()
         if cfg.use_depth_loss:
             self.depth_loss = DepthLoss(cfg.depth_loss_type)
             assert cfg.depth_lambda > 0, "depth_lambda should be > 0"
@@ -604,6 +610,87 @@ class DNSplatterModel(_ModelBase):
                 pred_normal=(2 * pred_normal - 1).permute(2, 0, 1), **extra)
         return {"main_loss": rgb_loss + reg, "scale_reg": scale_reg}
 
+    # ------------------------------------------------------------------ evaluation (reference :731-926)
+    def _eval_image(self, image: Tensor, outputs, keep_u8: bool) -> Tensor:
+        """A batch image as the metrics compare it, on the model's device: RGBA composited with the background; uint8
+        read as value / 255 (kept as stored when `keep_u8`, for the kernels to scale)."""
+        image = image.to(self.device)
+        if keep_u8 and image.dtype == torch.uint8 and image.shape[-1] == 3:
+            return image
+        background = outputs.get("background", self.background_color)
+        return self.composite_with_background(u8_as_float(image), background.to(self.device))
+
+    def _lpips(self, gt_rgb: Tensor, pred_rgb: Tensor, metrics_dict: Dict) -> None:
+        if callable(self.lpips):
+            metrics_dict["rgb_lpips"] = float(self.lpips(u8_as_float(gt_rgb).permute(2, 0, 1)[None],
+                                                         pred_rgb.permute(2, 0, 1)[None]))
+
+    def get_metrics_dict(self, outputs, batch) -> Dict[str, Union[float, int, Tensor]]:
+        """Reference dn_model.py:731-807: rgb_mse / rgb_psnr / rgb_ssim (rgb_lpips with `self.lpips` set),
+        gaussian_count, the depth_* metrics of the sensor depth when use_depth_loss, avg_min_scale.  While the training
+        resolution is downscaled, the image and sensor depth are resized as torchvision's TF.resize(antialias=None)
+        does (bilinear), not with the loss path's box filter."""
+        d = self._get_downscale_factor()
+        image, sensor_depth = batch["image"], batch.get("sensor_depth")
+        if d > 1:
+            image = tf_resize(image.permute(2, 0, 1), (image.shape[0] // d, image.shape[1] // d)).permute(1, 2, 0)
+            if sensor_depth is not None:
+                size = (sensor_depth.shape[0] // d, sensor_depth.shape[1] // d)
+                sensor_depth = tf_resize(sensor_depth.permute(2, 0, 1), size).permute(1, 2, 0)
+        gt_rgb = self._eval_image(image, outputs, keep_u8=True)
+        pred_rgb = outputs["rgb"][0, ...] if outputs["rgb"].dim() == 4 else outputs["rgb"]
+        mse, psnr, sim = rgb_metrics(pred_rgb.permute(2, 0, 1)[None], gt_rgb.permute(2, 0, 1)[None])
+        metrics_dict = {"rgb_mse": float(mse), "rgb_psnr": float(psnr), "rgb_ssim": float(sim)}
+        self._lpips(gt_rgb, pred_rgb, metrics_dict)
+        metrics_dict["gaussian_count"] = self.num_points
+        if self.config.use_depth_loss and sensor_depth is not None:
+            pred_depth = outputs["depth"][0, ...] if outputs["depth"].dim() == 4 else outputs["depth"]
+            values = self.depth_metrics(pred_depth.permute(2, 0, 1), sensor_depth.to(self.device).permute(2, 0, 1))
+            metrics_dict.update(_depth_dict(values))
+        metrics_dict["avg_min_scale"] = torch.nanmean(torch.exp(self.scales.detach()[..., -1]))
+        return metrics_dict
+
+    def get_image_metrics_and_images(self, outputs: Dict[str, Tensor], batch: Dict[str, Tensor]
+                                     ) -> Tuple[Dict[str, float], Dict[str, Tensor]]:
+        """Reference dn_model.py:809-926: rgb_psnr / rgb_ssim (rgb_lpips with `self.lpips` set), the depth_* metrics
+        when the batch has sensor_depth, normal_mae / normal_rsme (sic) / normal_mean_err / normal_med_err when it has
+        normal, and images_dict {img, depth, normal} with target and render side by side.  A batch mask multiplies
+        both images and both depths per pixel (the reference's [1,3,H,W] * [H,W,1] product fails for any real image).
+        The normal metrics compare the [0,1]-encoded maps as stored, as the reference does."""
+        dev = self.device
+        gt_rgb = self._eval_image(batch["image"], outputs, keep_u8=False)
+        pred_rgb = outputs["rgb"][0, ...] if outputs["rgb"].dim() == 4 else outputs["rgb"]
+        pred_depth = outputs["depth"][0, ...] if outputs["depth"].dim() == 4 else outputs["depth"]
+        pred_normal = outputs["normal"][0, ...] if outputs["normal"].dim() == 4 else outputs["normal"]
+        combined_rgb = torch.cat([gt_rgb, pred_rgb], dim=1)
+        combined_depth, combined_normal = pred_depth, pred_normal
+        mask = batch["mask"].to(dev) if "mask" in batch else None
+        if mask is not None:
+            gt_rgb, pred_rgb = gt_rgb * mask, pred_rgb * mask
+        _, psnr, sim = rgb_metrics(pred_rgb.permute(2, 0, 1)[None], gt_rgb.permute(2, 0, 1)[None])
+        metrics_dict = {"rgb_psnr": float(psnr), "rgb_ssim": float(sim)}
+        self._lpips(gt_rgb, pred_rgb, metrics_dict)
+        if "sensor_depth" in batch:
+            gt_depth = batch["sensor_depth"].to(dev)
+            if pred_depth.shape[:2] != gt_depth.shape[:2]:
+                pred_depth = tf_resize(pred_depth.permute(2, 0, 1), gt_depth.shape[:2]).permute(1, 2, 0)
+            gt_depth = gt_depth.to(torch.float32)
+            if mask is not None:
+                gt_depth, pred_depth = gt_depth * mask, pred_depth * mask
+            metrics_dict.update(_depth_dict(self.depth_metrics(pred_depth.permute(2, 0, 1), gt_depth.permute(2, 0, 1))))
+            combined_depth = torch.cat([gt_depth, pred_depth], dim=1)
+        if "normal" in batch:
+            gt_normal = u8_as_float(batch["normal"].to(dev))
+            pred_normal = pred_normal.to(dev)
+            if gt_normal.shape != pred_normal.shape:
+                pred_normal = tf_resize(pred_normal.permute(2, 0, 1), gt_normal.shape[:2]).permute(1, 2, 0)
+            mae, rmse, mean_err, med_err = self.normal_metrics(pred_normal.permute(2, 0, 1)[None],
+                                                               gt_normal.permute(2, 0, 1)[None])
+            metrics_dict.update({"normal_mae": float(mae), "normal_rsme": float(rmse), "normal_mean_err": float(mean_err),
+                                 "normal_med_err": float(med_err)})
+            combined_normal = torch.cat([gt_normal, pred_normal], dim=1)
+        return metrics_dict, {"img": combined_rgb, "depth": combined_depth, "normal": combined_normal}
+
     def step_cb(self, step: int):
         self.step = step
 
@@ -641,3 +728,8 @@ class DNSplatterModel(_ModelBase):
         state = self.__dict__.get("_densify_state") or DensifyState()
         self.__dict__["_densify_state"] = state
         return refinement_after(self, opts, step, state, self._densify_cfg(), self.num_train_data, generator)
+
+
+def _depth_dict(values) -> Dict[str, float]:
+    names = ("depth_abs_rel", "depth_sq_rel", "depth_rmse", "depth_rmse_log", "depth_a1", "depth_a2", "depth_a3")
+    return {k: float(v) for k, v in zip(names, values)}

@@ -2,11 +2,12 @@
 (/root/reference/dn_splatter/dn_pipeline.py:49-130): builds the datamanager, forwards seed points
 (points3D_xyz / points3D_rgb / points3D_normals metadata) to the model, and — where the reference wraps the
 model in DDP — installs the per-camera sharding + single flat all-reduce of parallel.py.
-Eval loops, point-cloud metrics and render dumps (dn_pipeline.py:133-638) are I/O around the hot path and
-out of scope (SURVEY.md §2.1 #6)."""
+get_average_eval_image_metrics averages the image metrics of every eval view (dn_pipeline.py:133-638); its point-cloud
+metrics, render dumps and MuSHRoom / FARO branches are not mirrored (SURVEY.md §2.1 #6)."""
 from __future__ import annotations
 
 from dataclasses import dataclass, field
+from time import time
 from typing import Any, Dict, Literal, Optional, Type
 
 import torch
@@ -94,3 +95,46 @@ class DNSplatterPipeline(_PipelineBase):
     def reduce_gradients(self):
         if self.bucket is not None:
             self.bucket.all_reduce()
+
+    @torch.no_grad()
+    def get_average_eval_image_metrics(self, step: Optional[int] = None, output_path=None, get_std: bool = False):
+        """Iterates over every eval image and averages the model's get_image_metrics_and_images over them, plus
+        num_rays_per_sec and fps of the render (reference dn_pipeline.py:133-638).  With `get_std`, every key also
+        gets `<key>_std` (torch.std_mean: NaN for a single image).
+
+        Datamanager contract: `datamanager.eval_dataset.cameras` is sliceable (cameras[i : i + 1] is view i) and
+        `datamanager.cached_eval` is a sequence of batches in the same order.  Point-cloud metrics
+        (skip_point_metrics=False; mesh_eval.point_cloud_metrics scores point clouds), render dumps (`output_path`) and
+        the MuSHRoom parser's split are not supported and raise NotImplementedError."""
+        if not self.config.skip_point_metrics:
+            raise NotImplementedError("point-cloud metrics in the eval loop: use mesh_eval.point_cloud_metrics")
+        if output_path is not None:
+            raise NotImplementedError("render dumps (output_path) are not supported")
+        if getattr(self.datamanager, "dataparser", None).__class__.__name__ == "MushroomDataParser":
+            raise NotImplementedError("the MuSHRoom with / within split of the eval metrics is not supported")
+        self.eval()
+        metrics_dict_list = []
+        cameras = self.datamanager.eval_dataset.cameras
+        for image_idx, batch in enumerate(self.datamanager.cached_eval):
+            camera = cameras[image_idx: image_idx + 1].to("cpu")
+            inner_start = time()
+            outputs = self.model.get_outputs_for_camera(camera=camera)
+            height, width = camera.height, camera.width
+            num_rays = height * width
+            metrics_dict, _ = self.model.get_image_metrics_and_images(outputs, batch)
+            assert "num_rays_per_sec" not in metrics_dict
+            metrics_dict["num_rays_per_sec"] = (num_rays / (time() - inner_start)).item()
+            assert "fps" not in metrics_dict
+            metrics_dict["fps"] = (metrics_dict["num_rays_per_sec"] / (height * width)).item()
+            metrics_dict_list.append(metrics_dict)
+        metrics_dict = {}
+        for key in metrics_dict_list[0].keys():
+            values = torch.tensor([m[key] for m in metrics_dict_list])
+            if get_std:
+                key_std, key_mean = torch.std_mean(values)
+                metrics_dict[key] = float(key_mean)
+                metrics_dict[f"{key}_std"] = float(key_std)
+            else:
+                metrics_dict[key] = float(torch.mean(values))
+        self.train()
+        return metrics_dict

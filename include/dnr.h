@@ -247,6 +247,14 @@ int dnr_ssim_fwd_ex(const float* pred, const void* gt, int32_t gt_is_u8, int32_t
 int dnr_ssim_bwd_ex(const float* pred, const void* gt, int32_t gt_is_u8, int32_t H, int32_t W, int32_t C, const float* dmaps,
                     const float* v_mean, float* v_pred, void* stream);
 
+/* Evaluation (no gradient) of the same SSIM for a batch, with the squared error for PSNR / MSE, as torchmetrics'
+ * StructuralSimilarityIndexMeasure(data_range=1.0, kernel_size=11) and PeakSignalNoiseRatio(data_range=1.0) need them
+ * (Python surface: dn_splatter_b200.metrics.RGBMetrics).  pred: [B,H,W,C] fp32; gt: [B,H,W,C] fp32, or uint8 read as
+ * value / 255 when gt_is_u8 != 0.  out [B,2] double (zeroed by the call): per image the SUM of the SSIM map over the
+ * (H-10)x(W-10) interior and all channels, and the sum of (pred - gt)^2 over all H*W*C values.  H, W >= 11; B <= 65535. */
+int dnr_rgb_metrics(const float* pred, const void* gt, int32_t gt_is_u8, int32_t B, int32_t H, int32_t W, int32_t C,
+                    double* out, void* stream);
+
 /* The whole photometric term of the parent SplatfactoModel.get_loss_dict [EXT] (dn_splatter/dn_model.py:624-628 calls it):
  *   main = (1 - ssim_lambda) * mean|pred - gt| + ssim_lambda * (1 - mean SSIM)
  * in one pass each way (the L1 sum shares the SSIM kernel's loads; its sign gradient is added by the SSIM backward).
@@ -435,6 +443,22 @@ int dnr_mesh_depth(const float* vertices /* [V,3] */, int32_t n_vertices, const 
 int dnr_mesh_visibility(const double* points /* [n,3] */, int64_t n_points, const double* cams /* [n_views,16] */,
                         const float* rendered, const float* gt, int32_t n_views, int32_t width, int32_t height, float eps,
                         int32_t* obs, int32_t* invalid, void* stream);
+
+/* ---- Render evaluation (Python surface: dn_splatter_b200.metrics; rules in csrc/metrics.cu and DESIGN.md) ----
+ * DepthMetrics (dn_splatter/metrics.py) over n pooled fp32 elements.  out[9] double (zeroed by the call), over the
+ * elements with gt > tolerance: [0] their count; [1], [2], [3] the counts of thresh < 1.25, 1.25^2, 1.25^3, where
+ * thresh = max(gt/pred, pred/gt) is formed in fp32 (NaN when either ratio is); [4] sum (gt-pred)^2; [5] sum |gt-pred|/gt;
+ * [6] sum (gt-pred)^2/gt; [7] sum |log gt - log pred| over the terms that are not NaN; [8] the number of those terms.
+ * Everything but the ratio test is evaluated in fp64. */
+int dnr_depth_metrics(const float* pred, const float* gt, int64_t n, float tolerance, double* out, void* stream);
+/* NormalMetrics (dn_splatter/metrics.py) of [B,H,W,3] maps: gt fp32, or uint8 read as value / 255 when gt_is_u8 != 0.
+ * out[3B+1] double (zeroed by the call): per image b, [3b] sum acos(clamp(dot, -1, 1)) with the fp32
+ * dot = (g0 p0 + g1 p1) + g2 p2, [3b+1] sum (g-p)^2, [3b+2] sum |g-p|; [3B] the lower median of the fp32 |g - p| over all
+ * N = 3BHW values (the element of rank (N-1)/2, as torch.median returns it), found by a radix select over the fp32 bit
+ * patterns without a host synchronisation.  ws: dnr_normal_metrics_workspace_bytes(B, H, W) bytes of device memory. */
+int64_t dnr_normal_metrics_workspace_bytes(int32_t B, int32_t H, int32_t W);
+int dnr_normal_metrics(const float* pred, const void* gt, int32_t gt_is_u8, int32_t B, int32_t H, int32_t W, void* ws,
+                       int64_t ws_bytes, double* out, void* stream);
 
 #ifdef __cplusplus
 }
