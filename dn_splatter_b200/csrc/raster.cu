@@ -25,6 +25,9 @@
 // operations with explicit rounding (V2 in common.cuh).  The backward's per-record warp reduction of its 16 gradient
 // values goes through a padded shared-memory transpose (4 STS.128 + 16 LDS.32 per lane, no SEL: fewer instructions than
 // a 16-SHFL / 30-SEL shuffle reduction), and is paid once per 128 pixels.
+//
+// Tests.  The forward is pinned per pixel (every output, last_ids, clamp_mask, depth_max) to the fp64 compositor of
+// oracle/raster_ref.py by tests/test_gpu_raster_forward.py; the backward by tests/test_gpu_backward_edges.py.
 #include "common.cuh"
 #include "loss_common.cuh"
 
