@@ -27,7 +27,9 @@
 // a 16-SHFL / 30-SEL shuffle reduction), and is paid once per 128 pixels.
 //
 // Tests.  The forward is pinned per pixel (every output, last_ids, clamp_mask, depth_max) to the fp64 compositor of
-// oracle/raster_ref.py by tests/test_gpu_raster_forward.py; the backward by tests/test_gpu_backward_edges.py.
+// oracle/raster_ref.py by tests/test_gpu_raster_forward.py; the backward per Gaussian (every grad_records slot, the
+// touched flags) to the fp64 backward of the same oracle by tests/test_gpu_raster_backward.py, and end to end by
+// tests/test_gpu_backward_edges.py.
 #include "common.cuh"
 #include "loss_common.cuh"
 

@@ -30,6 +30,10 @@ branches at such decisions; pixels with more than `max_alts` outcomes are listed
 
 `slip=` restates, in fp64, mistakes a kernel could make (SLIPS); tests/test_raster_ref_cpu.py uses them to show that the
 acceptance rule `judge` separates each of them from the correct result.
+
+`backward` differentiates `composite` at its own decisions with the conventions of `raster_bwd_kernel` and returns, per
+Gaussian, the 16 floats of a `grad_records` row with their absolute mass; `judge_bwd` is the per-Gaussian acceptance rule
+of tests/test_gpu_raster_backward.py, and BWD_SLIPS the backward mistakes tests/test_raster_bwd_ref_cpu.py holds it to.
 """
 from __future__ import annotations
 
@@ -141,8 +145,10 @@ def tile_box(means2d, radii):
 def composite(means2d, conics, opacities, colors, depths, normals_cam, radii, flatten_ids, tile_offsets, list_shift: int,
               width: int, height: int, background: Sequence[float], *, eps: float = 0.0, max_alts: int = 8,
               slip: Optional[str] = None, stale_depth_max: float = 0.0, tiles: Optional[Sequence[Tuple[int, int]]] = None,
-              chunk: int = 512) -> RasterRef:
-    """See the module docstring.  `tiles`: [(tx, ty)] restricts the work to those 16 x 16 tiles."""
+              chunk: int = 512, keep: Optional[dict] = None) -> RasterRef:
+    """See the module docstring.  `tiles`: [(tx, ty)] restricts the work to those 16 x 16 tiles.  `keep`: a dict that
+    receives, per walked tile (tx, ty), (y0, y1, x0, x1, g, pos, live[P,K], alpha[P,K], vis[P,K], dx[P,K], dy[P,K]) over
+    the K entries some pixel of the tile composited, in list order (`backward` differentiates exactly these)."""
     if slip is not None and slip not in SLIPS:
         raise ValueError(slip)
     m2, con, op = _np64(means2d), _np64(conics), _np64(opacities).reshape(-1)
@@ -194,6 +200,7 @@ def composite(means2d, conics, opacities, colors, depths, normals_cam, radii, fl
             cmarg = np.full(P, np.inf)
             clamped = np.zeros(P, bool)
             used = np.zeros(g_all.shape[0], bool)
+            kept = []
             for s in range(0, g_all.shape[0], chunk):
                 if fin.all():
                     break
@@ -203,7 +210,8 @@ def composite(means2d, conics, opacities, colors, depths, normals_cam, radii, fl
                 dy = m2[g, 1][None, :] - py[:, None]
                 t0, t1, t2 = 0.5 * con[g, 0][None] * dx * dx, 0.5 * con[g, 2][None] * dy * dy, con[g, 1][None] * dx * dy
                 sigma = (t0 + t1) + t2
-                ov = op[g][None, :] * np.exp(-sigma)
+                vis = np.exp(-sigma)
+                ov = op[g][None, :] * vis
                 alpha = np.minimum(ov, ALPHA_MAX)
                 valid = (sigma >= 0) & (alpha >= alpha_min)
                 a_eff = np.where(valid, alpha, 0.0)
@@ -222,6 +230,9 @@ def composite(means2d, conics, opacities, colors, depths, normals_cam, radii, fl
                 cand = np.where(live, pos[None, :], -1).max(1)
                 last = np.where(cand >= 0, cand, last)
                 used[s:s + chunk] |= live.any(0)
+                if keep is not None:
+                    cols = live.any(0)
+                    kept.append((g[cols], pos[cols], live[:, cols], alpha[:, cols], vis[:, cols], dx[:, cols], dy[:, cols]))
                 # margins of the decisions taken on the entries the pixel reached
                 den = np.abs(t0) + np.abs(t1) + np.abs(t2)
                 with np.errstate(invalid="ignore", divide="ignore"):
@@ -249,6 +260,8 @@ def composite(means2d, conics, opacities, colors, depths, normals_cam, radii, fl
                 kap = np.where(fin, kap, kap_new)
                 fin = fin | any_stop
             ref.n_contrib += int(used.sum())
+            if keep is not None and kept:
+                keep[(tx, ty)] = (y0, y1, x0, x1) + tuple(np.concatenate(k, axis=-1) for k in zip(*kept))
             sl = (slice(y0, y1), slice(x0, x1))
             ref.T[sl] = T.reshape(h, w_)
             ref.sums[sl] = acc.reshape(h, w_, 7)
@@ -461,3 +474,221 @@ def judge(ref: RasterRef, got: dict, eps: float, rtol: float, atol: float, regio
             n_used += 1
     return Verdict(worst=worst, worst_what=what, failures=failures, n_fail=n_fail, n_decided=int(decided.sum()),
                    n_ambiguous=n_amb, n_alt_used=n_used, n_unresolved=len(unresolved))
+
+
+# ------------------------------------------------------------------------------------------------------------ backward
+# kernel mistakes of `raster_bwd_kernel` restated in fp64 (`backward(slip=)`)
+BWD_SLIPS = (
+    "normal_to_means",  # the normal route's v_alpha reaches means2d (the normal pass sees detached means, quirk B3)
+    "abs_after_pair",   # |d/d means2d| taken after a lane's pixel pair (rows r and r + 2 of one column) is summed
+    "clamp_warp",       # the clamp fix-up zeroes the sigma / opacity gradient of every pixel of the warp (8-row half tile)
+    "clamp_missing",    # no clamp fix-up: a clamped pixel passes -op vis to sigma and vis to the opacity
+    "last_excluded",    # pos < last_id instead of pos <= last_id: the entry at last_id is skipped (gradient and T)
+    "no_bg",            # the -sum_k bg_k v_rgb_k term of v_alpha is dropped
+    "no_white_va",      # the white-background term -sum_c v_n_c of the normal image's v_alpha is dropped
+    "mask_ignored",     # the clamp mask is ignored: clamped rgb channels pass their upstream gradient
+    "no_depth_quot",    # the -v_depth D / alpha^2 term of v_alpha is dropped
+    "T_unclamped",      # T recovered back to front with 1 - op vis instead of 1 - min(op vis, 0.999)
+)
+SLOTS = ("x", "y", "|x|", "|y|", "A", "B", "C", "opacity", "r", "g", "b", "depth", "n0", "n1", "n2", "pad")
+
+
+@dataclass
+class RasterBwd:
+    """Outputs of `backward`: per Gaussian, the 16 floats of a `grad_records` row (include/dnr.h) and their scales."""
+
+    grads: np.ndarray  # [N,16] v_x, v_y, |v_x|, |v_y|, v_A, v_B, v_C, v_opacity, v_rgb, v_depth, v_n, 0
+    mass: np.ndarray   # [N,16] sum over pixels of the same expression with every term replaced by its absolute value
+    wmass: np.ndarray  # [N,16] the same sum, pixel p weighted by sqrt(1 + entries p composited)
+    tmass: np.ndarray  # [N,16] the same sum, pixel p weighted by |(1 - out_alpha) - T64_final| / T64_final
+    pix: np.ndarray    # [M] pixel index i * W + j of every (pixel, Gaussian) pair the forward composited
+    gid: np.ndarray    # [M] the Gaussian of that pair
+    fwd: RasterRef     # the forward oracle whose decisions were differentiated
+
+
+def backward(means2d, conics, opacities, colors, depths, normals_cam, radii, flatten_ids, tile_offsets, list_shift: int,
+             width: int, height: int, background: Sequence[float], v_rgb, v_depth, v_normal, v_alpha, state: dict, *,
+             replay: bool = True, slip: Optional[str] = None, tiles: Optional[Sequence[Tuple[int, int]]] = None,
+             pre: Optional[Tuple[RasterRef, dict]] = None) -> RasterBwd:
+    """fp64 gradient of sum(v_rgb rgb + v_depth depth + v_normal normal + v_alpha alpha) at the forward oracle's own
+    decisions (`composite`: which entries each pixel composited, where it stopped, the fp32 tile box), with the
+    conventions of `raster_bwd_kernel`:
+      * no gradient through sigma or opacity on a pixel where op vis > 0.999 (alpha is clamped there);
+      * an rgb channel outside [0, 1] before the clamp (clamp mask bit clear) passes nothing;
+      * the expected depth D / max(alpha, 1e-10) passes v_depth / alpha to D where alpha > 0 and -v_depth D / alpha^2
+        to alpha, with D / alpha read as the stored expected depth;
+      * the normal image (n / |n| + 1) / 2 of n = N + T (white background) is differentiated at the stored normal and
+        |n|; its route reaches conics and opacities but not means2d;
+      * |v_x|, |v_y| are sums over pixels of the absolute per-pixel derivative.
+    `state` holds the forward state the kernel reads: alpha, depth, normal, normal_norm, clamp_mask ([H,W(,3)]).
+    replay: the transmittances of each pixel are scaled so that T_final = 1 - state alpha, the value the kernel starts
+    its back-to-front recovery from; the result is then the exact derivative at that state.  Without it, the fp64 T.
+    Upstream images may be None (zero).  Slips: BWD_SLIPS.  `pre`: (ref, keep) of an earlier
+    `composite(..., keep=keep)` on the same inputs, reused instead of compositing again."""
+    if slip is not None and slip not in BWD_SLIPS:
+        raise ValueError(slip)
+    if pre is None:
+        keep: dict = {}
+        fwd = composite(means2d, conics, opacities, colors, depths, normals_cam, radii, flatten_ids, tile_offsets,
+                        list_shift, width, height, background, tiles=tiles, keep=keep)
+    else:
+        fwd, keep = pre
+    H, W = height, width
+    con, op = _np64(conics), _np64(opacities).reshape(-1)
+    N = con.shape[0]
+    normals = normals_cam is not None
+    feats = np.concatenate([_np64(colors), _np64(depths).reshape(-1, 1),
+                            _np64(normals_cam) if normals else np.zeros((N, 3))], 1)
+    bg = np.asarray(background, dtype=np.float64)
+    img = lambda x, s: np.zeros((H, W) + s) if x is None else _np64(x).reshape((H, W) + s)  # noqa: E731
+    g_rgb, g_d, g_a = img(v_rgb, (3,)), img(v_depth, ()), img(v_alpha, ())
+    g_n = img(v_normal if normals else None, (3,))
+    oa, od = img(state["alpha"], ()), img(state["depth"], ())
+    cmask = np.asarray(state["clamp_mask"]).astype(np.uint8).reshape(H, W)
+
+    # per pixel: the upstream gradient of the composited sums and of T_final (the kernel's prologue), and its mass
+    bit = (cmask[..., None] >> np.arange(3, dtype=np.uint8)) & 1
+    vC = g_rgb if slip == "mask_ignored" else np.where(bit == 1, g_rgb, 0.0)
+    ac = np.maximum(oa, 1e-10)
+    vD = np.where(oa > 0, g_d / ac, 0.0)
+    quot = np.where(oa >= 1e-10, g_d * od / ac, 0.0)
+    va_cd = g_a - (0.0 if slip == "no_bg" else (vC * bg).sum(-1)) - (0.0 if slip == "no_depth_quot" else quot)
+    mva_cd = np.abs(g_a) + (np.abs(vC) * np.abs(bg)).sum(-1) + np.abs(quot)
+    vN, mvN = np.zeros((H, W, 3)), np.zeros((H, W, 3))
+    va_n, mva_n = np.zeros((H, W)), np.zeros((H, W))
+    if normals:
+        nh = 2.0 * img(state["normal"], (3,)) - 1.0
+        nn = img(state["normal_norm"], ())[..., None]
+        gh = 0.5 * g_n
+        with np.errstate(invalid="ignore", divide="ignore"):
+            vN = (gh - nh * (nh * gh).sum(-1, keepdims=True)) / nn
+            mvN = (np.abs(gh) + np.abs(nh) * (np.abs(nh) * np.abs(gh)).sum(-1, keepdims=True)) / nn
+        if slip != "no_white_va":
+            va_n = -vN.sum(-1)
+        mva_n = mvN.sum(-1)
+    Tk = 1.0 - oa if replay else fwd.T
+    dT = np.abs((1.0 - oa) - fwd.T) / fwd.T
+    rw = np.sqrt(1.0 + fwd.ncomp)
+
+    out = {k: np.zeros((N, 16)) for k in ("grads", "mass", "wmass", "tmass")}
+    pix_l, gid_l = [], []
+
+    def later(x):  # sum over the entries after each one, along axis 1
+        c = np.flip(np.cumsum(np.flip(x, 1), 1), 1)
+        return np.concatenate([c[:, 1:], np.zeros((x.shape[0], 1))], 1)
+
+    for (y0, y1, x0, x1, g, pos, live, alpha, vis, dx, dy) in keep.values():
+        if g.shape[0] == 0:
+            continue
+        h, w_ = y1 - y0, x1 - x0
+        P = h * w_
+        sl = (slice(y0, y1), slice(x0, x1))
+        px = lambda a: a[sl].reshape((P,) + a.shape[2:])  # noqa: E731
+        p_idx = np.nonzero(live)
+        pix_l.append((y0 + p_idx[0] // w_) * W + x0 + p_idx[0] % w_)
+        gid_l.append(g[p_idx[1]])
+        if slip == "last_excluded":
+            live = live & (pos[None, :] != px(fwd.last_ids)[:, None])
+        a = np.where(live, alpha, 0.0)
+        ov = op[g][None, :] * vis
+        fac = np.where(live, 1.0 - ov, 1.0) if slip == "T_unclamped" else 1.0 - a
+        Tf = px(Tk)[:, None]
+        Tb = Tf / np.flip(np.cumprod(np.flip(fac, 1), 1), 1)  # T before each entry, recovered from T_final
+        wgt = a * Tb
+        inv = 1.0 / fac
+        f, af = feats[g], np.abs(feats[g])
+        vCp, vDp, vNp, mvNp = px(vC), px(vD), px(vN), px(mvN)
+        dot1 = vCp @ f[:, 0:3].T + vDp[:, None] * f[None, :, 3]
+        mdot1 = np.abs(vCp) @ af[:, 0:3].T + np.abs(vDp)[:, None] * af[None, :, 3]
+        dot2, mdot2 = vNp @ f[:, 4:7].T, mvNp @ af[:, 4:7].T
+        # d out / d alpha_i = T_i dot_i - (sum_{j>i} w_j dot_j - T_final va) / (1 - alpha_i), per route
+        va1 = Tb * dot1 - (later(wgt * dot1) - Tf * px(va_cd)[:, None]) * inv
+        mva1 = Tb * mdot1 + (later(wgt * mdot1) + Tf * px(mva_cd)[:, None]) * inv
+        va2 = Tb * dot2 - (later(wgt * dot2) - Tf * px(va_n)[:, None]) * inv
+        mva2 = Tb * mdot2 + (later(wgt * mdot2) + Tf * px(mva_n)[:, None]) * inv
+        clamped = live & (ov > ALPHA_MAX)
+        if slip == "clamp_missing":
+            zero = np.zeros_like(live)
+        elif slip == "clamp_warp":
+            half = (np.arange(P) // w_) >= 8
+            zero = np.where(half[:, None], clamped[half].any(0)[None, :], clamped[~half].any(0)[None, :])
+        else:
+            zero = clamped
+        nov = np.where(live & ~zero, -ov, 0.0)  # d alpha / d sigma
+        visg = np.where(live & ~zero, vis, 0.0)  # d alpha / d opacity
+        va, mva = va1 + va2, mva1 + mva2
+        vs, mvs = nov * va, -nov * mva
+        vs1, mvs1 = (vs, mvs) if slip == "normal_to_means" else (nov * va1, -nov * mva1)
+        A, B, Cc = con[g, 0][None, :], con[g, 1][None, :], con[g, 2][None, :]
+        gx, gy = vs1 * (A * dx + B * dy), vs1 * (B * dx + Cc * dy)
+        mgx, mgy = mvs1 * (np.abs(A * dx) + np.abs(B * dy)), mvs1 * (np.abs(B * dx) + np.abs(Cc * dy))
+        if slip == "abs_after_pair":  # rows r and r + 2 (r & 2 == 0) of a column share a lane's f32x2 pair
+            rows = np.arange(P) // w_
+            partner = np.where((rows & 2) == 0, np.arange(P) + 2 * w_, -1)
+            has = (partner >= 0) & (partner < P)
+            agx, agy = np.abs(gx), np.abs(gy)
+            for arr, gg in ((agx, gx), (agy, gy)):
+                arr[has] = np.abs(gg[has] + gg[partner[has]])
+                arr[partner[has]] = 0.0
+        else:
+            agx, agy = np.abs(gx), np.abs(gy)
+        vals = [gx, gy, agx, agy, 0.5 * vs * dx * dx, vs * dx * dy, 0.5 * vs * dy * dy, visg * va]
+        masses = [mgx, mgy, mgx, mgy, 0.5 * mvs * dx * dx, mvs * np.abs(dx * dy), 0.5 * mvs * dy * dy, visg * mva]
+        for k in range(3):
+            vals.append(wgt * vCp[:, k:k + 1])
+            masses.append(wgt * np.abs(vCp[:, k:k + 1]))
+        vals.append(wgt * vDp[:, None])
+        masses.append(wgt * np.abs(vDp)[:, None])
+        for k in range(3):
+            vals.append(wgt * vNp[:, k:k + 1])
+            masses.append(wgt * mvNp[:, k:k + 1])
+        r, t = px(rw)[:, None], px(dT)[:, None]
+        for k, (v, m) in enumerate(zip(vals, masses)):
+            m = np.where(live, m, 0.0)
+            np.add.at(out["grads"][:, k], g, np.where(live, v, 0.0).sum(0))
+            np.add.at(out["mass"][:, k], g, m.sum(0))
+            np.add.at(out["wmass"][:, k], g, (r * m).sum(0))
+            np.add.at(out["tmass"][:, k], g, (t * m).sum(0))
+    cat = lambda xs: np.concatenate(xs) if xs else np.zeros(0, np.int64)  # noqa: E731
+    return RasterBwd(pix=cat(pix_l), gid=cat(gid_l), fwd=fwd, **out)
+
+
+@dataclass
+class BwdVerdict:
+    worst: float         # largest |got - want| / bound over the judged Gaussians and slots
+    worst_what: str
+    failures: List[str]  # the first 10 failing (Gaussian, slot) reports
+    n_fail: int
+    n_judged: int        # Gaussians judged
+
+    @property
+    def ok(self) -> bool:
+        return self.n_fail == 0
+
+
+def bwd_bound(ref: RasterBwd, rtol: float, atol: float, extra: float = 0.0) -> np.ndarray:
+    """RTOL sum_p sqrt(1 + n_p) mass_pgk + ATOL max_g' mass_g'k (+ extra tmass: the T_final term of an unreplayed
+    reference)."""
+    return rtol * ref.wmass + atol * ref.mass.max(0, initial=0.0)[None, :] + extra * ref.tmass
+
+
+def judge_bwd(ref: RasterBwd, got: np.ndarray, rtol: float, atol: float, rows=None, extra: float = 0.0) -> BwdVerdict:
+    """Holds the kernel's grad_records `got` [N,16] to `ref` per Gaussian and slot.  A slot whose bound is 0 (no mass:
+    slot 15, the normal slots without v_normal, ...) must be exactly 0.  `rows`: bool [N] restricts the Gaussians."""
+    got = np.asarray(got, dtype=np.float64)
+    b = bwd_bound(ref, rtol, atol, extra)
+    err = np.abs(got - ref.grads)
+    with np.errstate(invalid="ignore", divide="ignore"):
+        ratio = np.where(err == 0, 0.0, err / b)
+    ratio = np.where(np.isnan(ratio), np.inf, ratio)
+    sel = np.ones(ratio.shape[0], bool) if rows is None else np.asarray(rows, bool)
+    rr = np.where(sel[:, None], ratio, -1.0)
+    bad = np.argwhere(rr > 1.0)
+    worst, what = 0.0, ""
+    if sel.any():
+        g, k = np.unravel_index(int(rr.argmax()), rr.shape)
+        worst = float(rr[g, k])
+        what = f"Gaussian {g} slot {k} ({SLOTS[k]}): got {got[g, k]:.9g}, want {ref.grads[g, k]:.9g}, bound {b[g, k]:.3g}"
+    fails = [f"Gaussian {g} slot {k} ({SLOTS[k]}): got {got[g, k]:.9g}, want {ref.grads[g, k]:.9g}, ratio {ratio[g, k]:.3g}"
+             for g, k in bad[:10]]
+    return BwdVerdict(worst=worst, worst_what=what, failures=fails, n_fail=int(bad.shape[0]), n_judged=int(sel.sum()))
