@@ -154,7 +154,10 @@ __device__ __forceinline__ HitGauss load_hit_gauss(const DnrArgs& a, const int32
       if (!(a.flags & DNR_FLAG_EXACT_LISTS)) {
         const float A = a.conics[h.g * 3 + 0], B = a.conics[h.g * 3 + 1], C = a.conics[h.g * 3 + 2];
         const float L = a.cull_lim[h.g];
-        const float det = A * C - B * B;
+        // A C - B^2 by Kahan's difference of products: for a needle (eps2d well below 0.3) the two products agree in
+        // all but their last bits, and the plain difference comes out <= 0 for a conic that is an ellipse
+        const float bb = B * B;
+        const float det = fmaf(A, C, -bb) + fmaf(-B, B, bb);
         if (!(L > 0.f) || !(det > 0.f)) {
           h.ny = 0;  // cannot reach alpha >= 1/255 anywhere
         } else {
