@@ -102,6 +102,27 @@ class DnrGridDesc(C.Structure):
 
 
 POISSON_MIN_DEPTH, POISSON_MAX_DEPTH, POISSON_MAX_CYCLES = 4, 10, 100
+ISO_POSE, ISO_MAX_DEPTH = 36, 10
+_d = C.c_double
+
+
+class DnrIsoFrames(C.Structure):
+    """Mirror of struct DnrIsoFrames (include/dnr.h)."""
+
+    _fields_ = [("depth", _p), ("normals", _p), ("poses", _p), ("n_frames", _i), ("width", _i), ("height", _i),
+                ("cam_normals", _i), ("K", _d * 9), ("inv_K", _d * 9), ("depth_scale", _d), ("rel_delta", _d)]
+
+
+class DnrIsoParams(C.Structure):
+    """Mirror of struct DnrIsoParams (include/dnr.h)."""
+
+    _fields_ = [("max_tsdf_rel", _d), ("max_tsdf_abs", _d), ("min_dot", _d), ("use_normals", _i), ("passes", _i)]
+
+
+class DnrIsoGrid(C.Structure):
+    """Mirror of struct DnrIsoGrid (include/dnr.h)."""
+
+    _fields_ = [("origin", _d * 3), ("cell", _d), ("max_depth", _i), ("threshold", _i)]
 
 
 POINTER_FIELDS = {n for n, t in DnrArgs._fields_ if t is _p}
@@ -120,6 +141,7 @@ KERNELS_PER_CALL = {
     "dnr_tsdf_integrate": (1, 0), "dnr_mc_count": (1, 6), "dnr_mc_emit": (2, 0),
     "dnr_grid_sample": (1, 0), "dnr_mesh_visibility": (1, 0),
     "dnr_rgb_metrics": (1, 0), "dnr_depth_metrics": (1, 0), "dnr_normal_metrics": (8, 0),
+    "dnr_iso_samples": (2, 2), "dnr_iso_eval": (1, 0), "dnr_iso_corners": (3, 4),
 }
 LAUNCHES = {"handwritten": 0, "cub": 0}
 DEBUG_CAPTURE = os.environ.get("DNR_DEBUG_CAPTURE") == "1"
@@ -281,6 +303,23 @@ def load():
     lib.dnr_bin_scan_workspace_bytes.argtypes = [C.c_int32]
     lib.dnr_bin_sort_workspace_bytes.restype = C.c_size_t
     lib.dnr_bin_sort_workspace_bytes.argtypes = [C.c_int32, C.c_int64, C.c_int32]
+    lib.dnr_iso_samples_workspace_bytes.restype = C.c_int64
+    lib.dnr_iso_samples_workspace_bytes.argtypes = [C.c_void_p, C.c_int32]
+    lib.dnr_iso_samples.restype = C.c_int
+    lib.dnr_iso_samples.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_iso_eval.restype = C.c_int
+    lib.dnr_iso_eval.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.dnr_iso_octree_workspace_bytes.restype = C.c_int64
+    lib.dnr_iso_octree_workspace_bytes.argtypes = [C.c_void_p, C.c_int64]
+    lib.dnr_iso_octree.restype = C.c_int
+    lib.dnr_iso_octree.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p]
+    lib.dnr_iso_corners_workspace_bytes.restype = C.c_int64
+    lib.dnr_iso_corners_workspace_bytes.argtypes = [C.c_void_p, C.c_int64]
+    lib.dnr_iso_corners.restype = C.c_int
+    lib.dnr_iso_corners.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                    C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_iso_fill.restype = C.c_int
+    lib.dnr_iso_fill.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = _Counting(lib)
     return _lib
 
@@ -294,7 +333,8 @@ EXPORTS = (
     "dnr_mc_emit_workspace_bytes", "dnr_mc_emit", "dnr_poisson_splat_workspace_bytes", "dnr_poisson_splat",
     "dnr_poisson_solve_workspace_bytes", "dnr_poisson_solve", "dnr_grid_sample", "dnr_mesh_depth_workspace_bytes",
     "dnr_mesh_depth", "dnr_mesh_visibility", "dnr_rgb_metrics", "dnr_depth_metrics", "dnr_normal_metrics_workspace_bytes",
-    "dnr_normal_metrics",
+    "dnr_normal_metrics", "dnr_iso_samples_workspace_bytes", "dnr_iso_samples", "dnr_iso_eval",
+    "dnr_iso_octree_workspace_bytes", "dnr_iso_octree", "dnr_iso_corners_workspace_bytes", "dnr_iso_corners", "dnr_iso_fill",
 )
 
 

@@ -31,6 +31,7 @@ SOURCES = {
     "poisson.cu": [],
     "mesh_eval.cu": ["-fmad=false"],  # visibility counts equal the fp64 oracle's
     "metrics.cu": ["-fmad=false"],  # per-element fp32 ratios, dots and |g - p| are restated exactly by the oracle
+    "isooctree.cu": ["-fmad=false"],  # fp64 samples and isoFunc values equal the oracle's bit for bit
 }
 
 

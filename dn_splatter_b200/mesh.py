@@ -234,6 +234,35 @@ def read_ply(path: str) -> TriangleMesh:
     return TriangleMesh(torch.from_numpy(verts), torch.from_numpy(f["i"].astype(np.int32).reshape(-1, 3)), torch.from_numpy(colors))
 
 
+def write_obj(path: str, mesh: TriangleMesh) -> None:
+    """Wavefront OBJ as isooctree_dn.py's writeMeshAsObj writes it: "v %f %f %f" lines, then 1-based "f %d %d %d"."""
+    verts = mesh.vertices.detach().cpu().double().numpy().reshape(-1, 3)
+    faces = mesh.faces.detach().cpu().numpy().astype(np.int64).reshape(-1, 3) + 1
+    with open(path, "wt") as fh:
+        if verts.shape[0]:
+            np.savetxt(fh, verts, fmt="v %f %f %f")
+        if faces.shape[0]:
+            np.savetxt(fh, faces, fmt="f %d %d %d")
+
+
+def read_obj(path: str) -> TriangleMesh:
+    """Vertices and triangles of an OBJ ("v x y z" and "f a b c" lines, 1-based, "a/t/n" forms allowed); no colours."""
+    verts, faces = [], []
+    with open(path) as fh:
+        for line in fh:
+            p = line.split()
+            if not p:
+                continue
+            if p[0] == "v":
+                verts.append([float(x) for x in p[1:4]])
+            elif p[0] == "f":
+                if len(p) != 4:
+                    raise ValueError(f"{path}: only triangle faces are supported")
+                faces.append([int(x.split("/")[0]) - 1 for x in p[1:4]])
+    return TriangleMesh(torch.tensor(verts, dtype=torch.float32).reshape(-1, 3),
+                        torch.tensor(faces, dtype=torch.int32).reshape(-1, 3), None)
+
+
 def _views(cameras) -> list:
     if isinstance(cameras, (list, tuple)):
         return list(cameras)

@@ -460,6 +460,66 @@ int64_t dnr_normal_metrics_workspace_bytes(int32_t B, int32_t H, int32_t W);
 int dnr_normal_metrics(const float* pred, const void* gt, int32_t gt_is_u8, int32_t B, int32_t H, int32_t W, void* ws,
                        int64_t ws_bytes, double* out, void* stream);
 
+/* ---- AGS-Mesh isooctree extraction (Python surface: dn_splatter_b200.isooctree; rules in csrc/isooctree.cu and
+ * DESIGN.md §2).  Everything that decides a sample or a value is evaluated in fp64.
+ *
+ * Frames: the depth and normal files of F views of one camera model (w x h, intrinsics K).  poses [F,DNR_ISO_POSE]
+ * (DEVICE doubles) per view: world->camera [3,4], camera->world rotation [3,3], camera position [3], normal rotation
+ * [3,3] (c2w rotation . diag(1, -1, -1), used when cam_normals != 0), all row-major, then 3 doubles of padding.  depth = file value * depth_scale;
+ * normals are the file values: uint8 PNG values of camera-frame normals (cam_normals != 0) or world-frame floats. */
+#define DNR_ISO_POSE 36
+#define DNR_ISO_MAX_DEPTH 10
+typedef struct DnrIsoFrames {
+  const float* depth;   /* [F,h,w] */
+  const float* normals; /* [F,h,w,3] */
+  const double* poses;  /* [F,DNR_ISO_POSE] */
+  int32_t n_frames, width, height, cam_normals;
+  double K[9], inv_K[9]; /* row-major */
+  double depth_scale;    /* 1/1000: millimetre files */
+  double rel_delta;      /* max_valid_depth_rel_delta (0.005) */
+} DnrIsoFrames;
+typedef struct DnrIsoParams {
+  double max_tsdf_rel;
+  double max_tsdf_abs; /* +inf: no absolute cap */
+  double min_dot;      /* cos(max_angle_to_max_weight_normal) */
+  int32_t use_normals;
+  int32_t passes; /* bit 0: a best-frame normal pass, bit 1: a fusion pass (3 = two-pass, 1 = choose_best_frame) */
+} DnrIsoParams;
+/* Octree over the hint cloud: root cube [origin, origin + cell * 2^max_depth)^3; a node splits iff it holds >= threshold
+ * samples and its level < max_depth.  Leaves: int64 level << 58 | Morton code of the node at its level (bit 3b + 2 - a
+ * is bit b of the axis-a coordinate), ordered by level, then code.  Lattice keys: (i * (R+1) + j) * (R+1) + k,
+ * R = 2^max_depth, sample (i, j, k) at origin + (i, j, k) * cell. */
+typedef struct DnrIsoGrid {
+  double origin[3];
+  double cell; /* finest cell edge */
+  int32_t max_depth; /* 0..DNR_ISO_MAX_DEPTH */
+  int32_t threshold; /* subdivision_threshold >= 1 */
+} DnrIsoGrid;
+/* The hint cloud (Frame.get_samples over all frames, in frame then row-major pixel order): points / normals (normals
+ * may be NULL) [capacity,3] with capacity = F * ceil(h/stride) * ceil(w/stride); *count_host = the survivors.
+ * Synchronises the stream (the one host read). */
+int64_t dnr_iso_samples_workspace_bytes(const DnrIsoFrames* frames, int32_t stride);
+int dnr_iso_samples(const DnrIsoFrames* frames, int32_t stride, void* ws, int64_t ws_bytes, double* points, double* normals,
+                    int64_t* count_host, void* stream);
+/* isoFunc at points [n,3]: values [n] (fp64 evaluation rounded to f32).  One thread per point, no host read. */
+int dnr_iso_eval(const DnrIsoFrames* frames, const DnrIsoParams* params, const double* points, int64_t n, float* values,
+                 void* stream);
+/* Leaves of the octree of points [n,3], kept in ws; level_counts_host[max_depth + 1] = leaves per level.  One host read
+ * per level. */
+int64_t dnr_iso_octree_workspace_bytes(const DnrIsoGrid* grid, int64_t n_points);
+int dnr_iso_octree(const DnrIsoGrid* grid, const double* points, int64_t n_points, void* ws, int64_t ws_bytes,
+                   int64_t* level_counts_host, void* stream);
+/* From dnr_iso_octree's workspace: leaves [L], the sorted unique corner lattice keys and their points (capacity 8L;
+ * *n_corners_host are written), leaf_corners [L,8] = the index of corner (dx << 2 | dy << 1 | dz) of each leaf. */
+int64_t dnr_iso_corners_workspace_bytes(const DnrIsoGrid* grid, int64_t n_leaves);
+int dnr_iso_corners(const DnrIsoGrid* grid, const void* octree_ws, const int64_t* level_counts_host, void* ws, int64_t ws_bytes,
+                    int64_t* leaves, int64_t* corner_keys, double* corner_points, int32_t* leaf_corners,
+                    int64_t* n_corners_host, void* stream);
+/* field [(R+1)^3] f32: every sample takes the value of the smallest leaf whose closed cube holds it, the lerp of lerps
+ * (x, then y, then z) of that leaf's corner values, which a corner sample reproduces exactly. */
+int dnr_iso_fill(const DnrIsoGrid* grid, const int64_t* leaves, const int64_t* level_counts_host, const int32_t* leaf_corners,
+                 const float* corner_values, float* field, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

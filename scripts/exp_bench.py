@@ -17,6 +17,10 @@ Rows (one JSON line each):
   mesh_eval   the TSDF mesh of that scene against its depth-9 `dn` Poisson mesh, 200 ring views at 1080p: CUDA-event
               times of depth rendering, visibility counts, subdivision, sampling and nearest neighbours, and the fp64
               numpy oracle's visibility counts and cKDTree metrics on a subset for scale
+  isooctree   export_isooctree_mesh's stages on the same scene, 200 ring views at 1080p, pixel_stride 6, max_depth 10:
+              render into the frame buffers, hint cloud, octree + corners, isoFunc at the corners, dense fill, marching
+              cubes (CUDA events), and the fp64 numpy oracle's isoFunc rate (point-frame evaluations per second) on a
+              subset for scale
 Each row also checks agreement with the reference path (max abs / rel error), so a faster-but-wrong kernel is visible.
 """
 import argparse
@@ -491,9 +495,79 @@ def bench_mesh_eval():
     emit(row)
 
 
+def bench_isooctree():
+    import subprocess
+    import time
+
+    import numpy as np
+
+    from dn_splatter_b200 import isooctree as I
+    from dn_splatter_b200.cameras import Cameras
+    from dn_splatter_b200.dn_model import DNSplatterModelConfig
+    from dn_splatter_b200.mesh import marching_cubes
+    from dn_splatter_b200.synthetic import make_scene, ring_cameras
+    from oracle import isooctree_ref as R
+
+    W, H, n_views, stride, depth, thr = 1920, 1080, 200, 6, 10, 50
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip().splitlines()[0]
+    m = DNSplatterModelConfig(random_init=True, num_random=16, background_color="black", sync_free=True).setup(device="cuda")
+    m.load_gaussians(make_scene(args.n, seed=0))
+    m.step = 30000
+    cams = [Cameras(c["c2w"][None], c["fx"], c["fy"], c["cx"], c["cy"], W, H) for c in ring_cameras(n_views, W, H)]
+    row = {"row": "isooctree", "card": card, "n_gauss": args.n, "views": n_views, "resolution": f"{W}x{H}",
+           "pixel_stride": stride, "max_depth": depth, "subdivision_threshold": thr}
+    I.render_frames(m, cams[:4])  # warm-up: captures the forward graphs
+    ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
+    e = [ev() for _ in range(7)]
+    torch.cuda.synchronize()
+    e[0].record()
+    fs = I.render_frames(m, cams)
+    e[1].record()
+    hint, _ = I.hint_samples(fs, stride)
+    e[2].record()
+    tree = I.build_octree(hint, depth, thr)
+    e[3].record()
+    values = I.iso_eval(fs, tree.corner_points)
+    e[4].record()
+    field = I.fill_grid(tree, values)
+    e[5].record()
+    mesh = marching_cubes(field, 0.0, tree.origin, tree.cell)
+    e[6].record()
+    torch.cuda.synchronize()
+    for k, name in enumerate(("render", "hint", "octree", "eval", "fill", "marching_cubes")):
+        row[f"{name}_ms"] = e[k].elapsed_time(e[k + 1])
+    row["hint_samples"], row["leaves"], row["corners"] = int(hint.shape[0]), int(tree.leaves.shape[0]), int(values.shape[0])
+    row["triangles"] = int(mesh.faces.shape[0])
+    row["eval_point_frames_per_s"] = values.shape[0] * n_views / (row["eval_ms"] * 1e-3)
+    row["fill_gsamples_per_s"] = field.numel() / (row["fill_ms"] * 1e-3) / 1e9
+    del field, mesh
+    torch.cuda.empty_cache()
+    nf, npt = 4, 20_000  # the oracle on a subset: its cost is linear in points x frames
+    cam = R.CameraModel({"w": W, "h": H, "fl_x": float(cams[0].fx), "fl_y": float(cams[0].fy), "cx": float(cams[0].cx),
+                         "cy": float(cams[0].cy)})
+    frames = []
+    for k in range(nf):
+        c2w = np.eye(4)  # the pose row's c2w rotation and position; transform_matrix @ CAM_CONVENTION_CHANGE gives it back
+        c2w[:3, :3], c2w[:3, 3] = fs._poses[k][12:21].reshape(3, 3), fs._poses[k][21:24]
+        frames.append(R.Frame(cam, c2w @ R.CAM_CONVENTION_CHANGE, fs.depth[k].cpu().numpy(),
+                              fs.normals[k].cpu().numpy().astype(np.uint8), True))
+    pts = tree.corner_points[:npt].cpu().numpy()
+    t0 = time.perf_counter()
+    ref = R.iso_func(frames, pts)
+    row["oracle_point_frames_per_s"] = npt * nf / (time.perf_counter() - t0)
+    sub = I.FrameSet(fs.camera, nf, True)
+    sub.depth.copy_(fs.depth[:nf])
+    sub.normals.copy_(fs.normals[:nf])
+    sub._poses[:] = fs._poses[:nf]
+    got = I.iso_eval(sub, tree.corner_points[:npt]).cpu().numpy()
+    row["eval_max_abs_err_vs_oracle"] = float(np.abs(got - ref).max())
+    emit(row)
+
+
 for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("camera_opt", bench_camera_opt), ("knn", bench_knn),
                  ("render_service", bench_render_service), ("mesh", bench_mesh), ("poisson", bench_poisson),
-                 ("mesh_eval", bench_mesh_eval)):
+                 ("mesh_eval", bench_mesh_eval), ("isooctree", bench_isooctree)):
     if args.only and name not in args.only.split(","):
         continue
     try:
