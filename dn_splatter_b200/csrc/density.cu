@@ -10,7 +10,8 @@
 // reused for the 21 samples).  Precise expf / division: this is an export-time path compared value by value.
 //
 // The algorithm is pinned on the CPU (oracle/sugar_ref.py vs goldens from the reference's own functions) and the kernel
-// against that restatement on the GPU (tests/test_gpu_sugar.py).
+// against that restatement on the GPU (tests/test_gpu_sugar.py), and per sample / per ray against an fp64 sum with a
+// per-term error bound (tests/test_gpu_knn_density.py).
 #include "common.cuh"
 
 namespace {
@@ -74,10 +75,12 @@ __global__ void __launch_bounds__(256) density_kernel(const float* __restrict__ 
   out[i] = fmaxf(squash(d), clamp_min);
 }
 
-// torch.linspace(-R, R, 21) in fp32: start + i*step below the midpoint, end - (20-i)*step from it on
+// torch.linspace(-R, R, 21) in fp32: start + i*step below the midpoint, end - (20-i)*step from it on, each rounded once
+// as torch's fused multiply-add does (this file is built with -fmad=false, so the fma is spelled out: two roundings
+// differ from torch at 5 of the 21 samples for R = 3)
 __device__ __forceinline__ float linspace21(int i, float range) {
   const float step = (range - (-range)) / 20.0f;
-  return i < RAY_SAMPLES / 2 ? -range + step * (float)i : range - step * (float)(RAY_SAMPLES - 1 - i);
+  return i < RAY_SAMPLES / 2 ? fmaf(step, (float)i, -range) : fmaf(-step, (float)(RAY_SAMPLES - 1 - i), range);
 }
 
 __global__ void __launch_bounds__(128) ray_density_kernel(const float* __restrict__ points, int64_t P, const int64_t* __restrict__ idx, int k,

@@ -4,14 +4,23 @@
 // k_nearest_sklearn used by populate_modules (dn_model.py:187) [EXT].
 //
 // Build: points are binned into a uniform grid (origin / cell size / dims chosen by the host from the point statistics;
-// points outside the box are clamped into the border cells, which keeps the search exact — see the bound below), sorted by
-// cell with cub, and each cell's [start, end) range recorded.  Query: one thread per query walks cube shells of growing
-// Chebyshev radius r around its own (clamped) cell, keeping the K best in a sorted per-thread list.  Because the
-// coordinate -> cell map is monotone per axis, two points whose cells differ by D along an axis are at least (D-1) cells
-// apart, so after shell r everything unvisited is >= r * cell away: the search stops once the K-th distance <= r * cell.
+// points outside the box are clamped into the border cells, which keeps the bound below valid), sorted by cell with cub,
+// and each cell's [start, end) range recorded.  Query: one thread per query walks cube shells of growing Chebyshev radius
+// r around its own (clamped) cell, keeping the K best in a sorted per-thread list.
 //
-// Pinned on the CPU by a numpy mirror against sklearn (tests/test_knn_grid_cpu.py) and on the GPU against a brute-force
-// fp64 distance matrix (tests/test_gpu_sugar.py).
+// Stop rule.  In exact arithmetic the coordinate -> cell map u = (x - lo) / cell is monotone per axis, so two points whose
+// cells differ by D along an axis are more than (D-1) cells apart and, after shell r, everything unvisited is > r * cell
+// away.  The kernel bins by fl(fl(x - lo) * inv_cell) in fp32: three roundings (the difference, inv_cell = fl(1 / cell),
+// the product), so u is off by at most 4 eps |u| (eps = 2^-24, one more for a host that rounds 1 / cell twice).  Along
+// the axis where the cells differ by r+1 the computed gap exceeds r, the larger u is >= 1 and the smaller one < dim, so
+// the true gap exceeds r (1 - 4 eps) - 8 eps dim >= r - 12 eps max_dim cells (r < dim).  The search
+// therefore stops only once the K-th distance <= (r - delta) * cell with delta = 2^-18 max_dim, 5.3x that bound (about
+// 1e-3 cells at the 256-cell cap of choose_grid; measured binning errors reach 2.4e-5 cells there).  What remains is the
+// fp32 rounding of the distances themselves: a returned neighbour is farther than an unreturned one only when their
+// squared distances agree to about 10 eps relative, the band inside which fp32 cannot order them anyway.
+//
+// Pinned on the CPU by a numpy mirror against sklearn (tests/test_knn_grid_cpu.py) and on the GPU per query against
+// brute-force fp64 distances (tests/test_gpu_knn_density.py).
 #include <cub/cub.cuh>
 
 #include "common.cuh"
@@ -114,6 +123,7 @@ __global__ void __launch_bounds__(128) knn_query_kernel(const float* __restrict_
   const int cy = cell_coord(qy, g.lo[1], g.inv_cell, g.dims[1]);
   const int cz = cell_coord(qz, g.lo[2], g.inv_cell, g.dims[2]);
   const int r_max = max(max(max(cx, g.dims[0] - 1 - cx), max(cy, g.dims[1] - 1 - cy)), max(cz, g.dims[2] - 1 - cz));
+  const float delta = (float)max(max(g.dims[0], g.dims[1]), g.dims[2]) * 0x1p-18f;  // binning slack in cells (see top)
   TopK t;
   t.count = 0;
   for (int r = 0; r <= r_max; ++r) {
@@ -133,7 +143,7 @@ __global__ void __launch_bounds__(128) knn_query_kernel(const float* __restrict_
         }
       }
     }
-    const float reach = (float)r * g.cell;
+    const float reach = fmaxf((float)r - delta, 0.f) * g.cell;
     if (t.count == K && t.d[K - 1] <= reach * reach) break;
   }
   const int k_out = K - skip;

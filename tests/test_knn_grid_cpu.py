@@ -36,6 +36,7 @@ def query(points, g, order, start, end, q, K, skip):
     c = np.clip(np.floor((q - lo) * inv).astype(np.int64), 0, np.array(dims) - 1)
     cx, cy, cz = int(c[0]), int(c[1]), int(c[2])
     r_max = max(cx, dims[0] - 1 - cx, cy, dims[1] - 1 - cy, cz, dims[2] - 1 - cz)
+    delta = np.float32(max(dims)) * np.float32(2.0 ** -18)  # the fp32 binning slack, in cells
     d, ids = [], []
 
     def insert(d2, i):
@@ -73,8 +74,8 @@ def query(points, g, order, start, end, q, K, skip):
                     if cx + r < dims[0]:
                         scan(row + cx + r)
                         visited += 1
-        reach = np.float32(r) * cellf
-        if len(d) == K and d[K - 1] <= reach * reach:
+        reach = max(np.float32(r) - delta, np.float32(0)) * cellf
+        if len(d) == K and d[K - 1] <= np.float32(reach * reach):
             break
     return ids[skip:], visited
 
@@ -119,6 +120,28 @@ def test_grid_search_equals_sklearn(name):
             visited_in.append(visited)
     if name != "tiny":  # the bound prunes: queries near the data touch a small part of the grid
         assert np.mean(visited_in) < 0.35 * total_cells, (np.mean(visited_in), total_cells)
+
+
+# Binning in fp32 moves cell boundaries: the query lands at u = 158.99998 (cell 158), A at 160.0 (cell 160), B at
+# 157.99998 (cell 157).  A is nearer than B by 5.4e-6 relative, far outside the fp32 tie band, but A sits two cells
+# away and B only one, so a stop rule of "K-th distance <= r * cell" returns B after shell 1.
+STOP_RULE_GRID = {"lo": [-2.3644726, 0.0, 0.0], "cell": 0.013844357633743604, "dims": [256, 1, 1]}
+STOP_RULE_POINTS = [[-0.14937554, 0.0, 0.0], [-0.17706418, 0.0, 0.0]]  # A (nearest), B
+STOP_RULE_QUERY = [-0.16321982, 0.0, 0.0]
+
+
+def test_stop_rule_covers_the_fp32_binning_error():
+    pts = np.array(STOP_RULE_POINTS, np.float32)
+    q = np.array(STOP_RULE_QUERY, np.float32)
+    g = STOP_RULE_GRID
+    inv = np.float32(1.0 / g["cell"])
+    u = [float(np.float32(np.float32(x - np.float32(g["lo"][0])) * inv)) for x in (q[0], pts[0, 0], pts[1, 0])]
+    assert [math.floor(v) for v in u] == [158, 160, 157]  # the case still straddles the cells as described
+    d = np.abs(pts[:, 0].astype(np.float64) - float(q[0]))
+    assert d[0] < d[1] * (1 - 5e-6)
+    order, start, end = build(pts, g)
+    got, _ = query(pts, g, order, start, end, q, 1, skip=0)
+    assert got == [0]
 
 
 def test_fewer_points_than_k():
