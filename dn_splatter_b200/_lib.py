@@ -125,6 +125,21 @@ class DnrIsoGrid(C.Structure):
     _fields_ = [("origin", _d * 3), ("cell", _d), ("max_depth", _i), ("threshold", _i)]
 
 
+DN_MAX_K, DN_OMNIDATA, DN_DSINE, DN_DEPTH_TO_NORMAL = 256, 0, 1, 2
+
+
+class DnrDnPose(C.Structure):
+    """Mirror of struct DnrDnPose (include/dnr.h)."""
+
+    _fields_ = [("rinv", _d * 9), ("t", _d * 3)]
+
+
+class DnrDnSearch(C.Structure):
+    """Mirror of struct DnrDnSearch (include/dnr.h)."""
+
+    _fields_ = [("lo", _d * 3), ("cell", _d), ("center", _d * 3), ("k", _i), ("orient", _i)]
+
+
 POINTER_FIELDS = {n for n, t in DnrArgs._fields_ if t is _p}
 
 _lib: Optional[C.CDLL] = None
@@ -142,6 +157,7 @@ KERNELS_PER_CALL = {
     "dnr_grid_sample": (1, 0), "dnr_mesh_visibility": (1, 0),
     "dnr_rgb_metrics": (1, 0), "dnr_depth_metrics": (1, 0), "dnr_normal_metrics": (8, 0),
     "dnr_iso_samples": (2, 2), "dnr_iso_eval": (1, 0), "dnr_iso_corners": (3, 4),
+    "dnr_dn_backproject": (1, 0), "dnr_dn_normals": (8, 5), "dnr_dn_consistency": (1, 0),
 }
 LAUNCHES = {"handwritten": 0, "cub": 0}
 DEBUG_CAPTURE = os.environ.get("DNR_DEBUG_CAPTURE") == "1"
@@ -320,6 +336,16 @@ def load():
                                     C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dnr_iso_fill.restype = C.c_int
     lib.dnr_iso_fill.argtypes = [C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_dn_backproject.restype = C.c_int
+    lib.dnr_dn_backproject.argtypes = [C.c_void_p, C.c_int32, C.c_int32, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_dn_normals_workspace_bytes.restype = C.c_int64
+    lib.dnr_dn_normals_workspace_bytes.argtypes = [C.c_int64]
+    lib.dnr_dn_normals.restype = C.c_int
+    lib.dnr_dn_normals.argtypes = [C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_void_p, C.c_void_p,
+                                   C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_dn_consistency.restype = C.c_int
+    lib.dnr_dn_consistency.argtypes = [C.c_void_p, C.c_void_p, C.c_int64, C.c_void_p, C.c_int32, C.c_double, C.c_void_p,
+                                       C.c_void_p, C.c_void_p, C.c_void_p]
     _lib = _Counting(lib)
     return _lib
 
@@ -335,6 +361,7 @@ EXPORTS = (
     "dnr_mesh_depth", "dnr_mesh_visibility", "dnr_rgb_metrics", "dnr_depth_metrics", "dnr_normal_metrics_workspace_bytes",
     "dnr_normal_metrics", "dnr_iso_samples_workspace_bytes", "dnr_iso_samples", "dnr_iso_eval",
     "dnr_iso_octree_workspace_bytes", "dnr_iso_octree", "dnr_iso_corners_workspace_bytes", "dnr_iso_corners", "dnr_iso_fill",
+    "dnr_dn_backproject", "dnr_dn_normals_workspace_bytes", "dnr_dn_normals", "dnr_dn_consistency",
 )
 
 

@@ -32,6 +32,7 @@ SOURCES = {
     "mesh_eval.cu": ["-fmad=false"],  # visibility counts equal the fp64 oracle's
     "metrics.cu": ["-fmad=false"],  # per-element fp32 ratios, dots and |g - p| are restated exactly by the oracle
     "isooctree.cu": ["-fmad=false"],  # fp64 samples and isoFunc values equal the oracle's bit for bit
+    "normals.cu": ["-fmad=false"],  # fp32 camera coordinates and uint8 encodings equal numpy's bit for bit
 }
 
 

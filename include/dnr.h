@@ -520,6 +520,45 @@ int dnr_iso_corners(const DnrIsoGrid* grid, const void* octree_ws, const int64_t
 int dnr_iso_fill(const DnrIsoGrid* grid, const int64_t* leaves, const int64_t* level_counts_host, const int32_t* leaf_corners,
                  const float* corner_values, float* field, void* stream);
 
+/* ---- AGS-Mesh depth confidence masks: scripts/depth_normal_consistency.py and depth_to_normal.py (DESIGN.md §2 (9)) ---- */
+#define DNR_DN_MAX_K 256
+#define DNR_DN_OMNIDATA 0         /* DepthNormalConsistency, normal_format "omnidata" */
+#define DNR_DN_DSINE 1            /* DepthNormalConsistency, normal_format "dsine" */
+#define DNR_DN_DEPTH_TO_NORMAL 2  /* DepthToNormal: the angle between the encoded vectors */
+/* A 3x3 matrix (row-major) and a translation.  dnr_dn_backproject: world = cam @ rinv + t with rinv = inv(c2w[:3,:3]);
+ * dnr_dn_consistency: rinv holds R = transpose(inv(c2w)[:3,:3]), the mono normal's rotation, and t is unused. */
+typedef struct DnrDnPose {
+  double rinv[9];
+  double t[3];
+} DnrDnPose;
+/* The neighbour search: k in [1, DNR_DN_MAX_K]; the Morton grid spans lo + [0, 2^21 cell) per axis (points outside are
+ * clamped into the border cells); with orient != 0 a normal n of point p is negated where (p - center) . n > 0. */
+typedef struct DnrDnSearch {
+  double lo[3];
+  double cell;
+  double center[3];
+  int32_t k;
+  int32_t orient;
+} DnrDnSearch;
+/* points [w*h,3] f64 of a depth frame [h,w] f32 (intrinsics_host = fx, fy, cx, cy as f32); cam_points [w*h,3] f32, the
+ * camera coordinates, may be NULL. */
+int dnr_dn_backproject(const float* depth, int32_t width, int32_t height, const float* intrinsics_host, const DnrDnPose* pose,
+                       float* cam_points, double* points, void* stream);
+/* normals [n,3] f64 of points [n,3] f64 (Open3D's estimate_normals, KNN k, fast_normal_computation) [EXT].  Optional
+ * outputs (NULL: not written): examined [n] the candidates the search of each point's position examined; stats (device,
+ * 2 x u64) += (candidates examined, searches run), one search per distinct position; for tests, cov [n,9] the covariance of
+ * each point's neighbours and neighbours [n,k] the smallest point index of each neighbour's position, one entry per copy
+ * taken, -1 past min(k, n). */
+/* The cub scratch in the workspace is sized by cub's queries, which need a device; without one they fail and the size
+ * returned lacks that scratch.  dnr_dn_normals repeats the queries and returns their cudaError_t (> 0) if they fail. */
+int64_t dnr_dn_normals_workspace_bytes(int64_t n_points);
+int dnr_dn_normals(const double* points, int64_t n_points, const DnrDnSearch* search, void* ws, int64_t ws_bytes, double* normals,
+                   int32_t* examined, double* cov, int32_t* neighbours, unsigned long long* stats, void* stream);
+/* Per pixel of oriented normals [n,3] and the mono-normal PNG values mono [n,3] u8: the angle in degrees, mask = 255 where it
+ * exceeds threshold else 0, and normals_u8 [n,3] = uint8((n + 1) / 2 * 255). */
+int dnr_dn_consistency(const double* normals, const uint8_t* mono, int64_t n, const DnrDnPose* rotation, int32_t mode,
+                       double threshold, double* degrees, uint8_t* mask, uint8_t* normals_u8, void* stream);
+
 #ifdef __cplusplus
 }
 #endif

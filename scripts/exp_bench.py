@@ -21,6 +21,10 @@ Rows (one JSON line each):
               render into the frame buffers, hint cloud, octree + corners, isoFunc at the corners, dense fill, marching
               cubes (CUDA events), and the fp64 numpy oracle's isoFunc rate (point-frame evaluations per second) on a
               subset for scale
+  depth_normals  DepthNormalConsistency's per-frame device work on a room frame (0.3-8 m, 5 % / 40 % holes in blobs) at
+              1920x1440 and 1024x768, k = 200: back-projection, normals (k-NN + covariance + FastEigen3x3 + orientation)
+              and the consistency pass (CUDA events), candidates examined per search (mean) and per surface pixel (mean,
+              p99), and the fp64 numpy oracle's rate on a 64x48 crop for scale
 Each row also checks agreement with the reference path (max abs / rel error), so a faster-but-wrong kernel is visible.
 """
 import argparse
@@ -565,9 +569,84 @@ def bench_isooctree():
     emit(row)
 
 
+def bench_depth_normals():
+    import subprocess
+    import time
+
+    import numpy as np
+
+    from dn_splatter_b200 import depth_normals as DN
+    from oracle import normals_ref as R
+
+    card = subprocess.run(["nvidia-smi", "--query-gpu=name,power.limit", "--format=csv,noheader"], capture_output=True,
+                          text=True).stdout.strip().splitlines()[0]
+
+    def room(w, h, share, seed=0):
+        g = np.random.default_rng(seed)
+        u, v = np.meshgrid(np.arange(w) / w, np.arange(h) / h)
+        z = 0.3 + 7.7 * u ** 2 + 0.3 * np.sin(v * 6)  # 0.3-8 m across the frame
+        hw, hh = w // 8, h // 8  # holes as blobs on a coarse grid, upsampled
+        hu, hv = np.meshgrid(np.arange(hw), np.arange(hh))
+        holes = np.zeros((hh, hw), bool)
+        while holes.mean() < share:
+            cx, cy, r = g.integers(0, hw), g.integers(0, hh), g.integers(1, max(2, hw // 20))
+            holes |= (hu - cx) ** 2 + (hv - cy) ** 2 < r * r
+        holes = np.repeat(np.repeat(holes, 8, 0), 8, 1)[:h, :w]
+        return np.where(holes, 0, z).astype(np.float32)
+
+    reps = 3
+    for (w, h) in ((1920, 1440), (1024, 768)):
+        for share in (0.05, 0.40):
+            depth = room(w, h, share)
+            intr = (0.73 * w, 0.73 * w, w / 2, h / 2)
+            c2w = np.eye(4)
+            mono = np.random.default_rng(1).integers(0, 256, (h * w, 3)).astype(np.uint8)
+            n = w * h
+            examined = torch.empty(n, dtype=torch.int32, device="cuda")
+            stats = torch.zeros(2, dtype=torch.int64, device="cuda")
+            ev = lambda: torch.cuda.Event(enable_timing=True)  # noqa: E731
+            pts = DN.backproject_depth(depth, *intr, c2w)  # warm-up
+            DN.depth_normal_consistency(DN.estimate_normals(pts, 200, c2w[:3, 3]), mono, c2w)
+            t = {"backproject": 0.0, "normals": 0.0, "consistency": 0.0}
+            for r in range(reps):
+                e = [ev() for _ in range(4)]
+                torch.cuda.synchronize()
+                e[0].record()
+                pts = DN.backproject_depth(depth, *intr, c2w)
+                e[1].record()
+                nrm = DN.estimate_normals(pts, 200, c2w[:3, 3], stats=stats if r == 0 else None,
+                                          examined=examined if r == 0 else None)
+                e[2].record()
+                DN.depth_normal_consistency(nrm, mono, c2w)
+                e[3].record()
+                torch.cuda.synchronize()
+                for k, name in enumerate(t):
+                    t[name] += e[k].elapsed_time(e[k + 1]) / reps
+            s = stats.cpu().numpy()
+            ex = examined.cpu().numpy()[depth.reshape(-1) > 0]
+            row = {"row": "depth_normals", "card": card, "resolution": f"{w}x{h}", "holes": share, "k": 200,
+                   "hole_share_measured": float((depth == 0).mean()), **{f"{k}_ms": v for k, v in t.items()},
+                   "frame_ms": sum(t.values()), "searches": int(s[1]),
+                   "candidates_per_search_mean": float(s[0] / s[1]),
+                   "candidates_per_surface_pixel_mean": float(ex.mean()),
+                   "candidates_per_surface_pixel_p99": float(np.percentile(ex, 99))}
+            if (w, h) == (1024, 768) and share == 0.05:  # the oracle on a crop, for scale
+                crop = pts.reshape(h, w, 3)[360:408, 480:544].reshape(-1, 3).cpu().numpy()
+                t0 = time.perf_counter()
+                ref, _ = R.estimate_normals(crop, 200)
+                row["oracle_points_per_s"] = crop.shape[0] / (time.perf_counter() - t0)
+                got = DN.estimate_normals(torch.from_numpy(crop).cuda(), 200).cpu().numpy()
+                row["crop_max_abs_err_vs_oracle_up_to_sign"] = float(np.minimum(np.abs(got - ref).max(1),
+                                                                               np.abs(got + ref).max(1)).max())
+            emit(row)
+            del pts, nrm, examined
+            torch.cuda.empty_cache()
+
+
 for name, fn in (("ssim", bench_ssim), ("adam", bench_adam), ("camera_opt", bench_camera_opt), ("knn", bench_knn),
                  ("render_service", bench_render_service), ("mesh", bench_mesh), ("poisson", bench_poisson),
-                 ("mesh_eval", bench_mesh_eval), ("isooctree", bench_isooctree)):
+                 ("mesh_eval", bench_mesh_eval), ("isooctree", bench_isooctree),
+                 ("depth_normals", bench_depth_normals)):
     if args.only and name not in args.only.split(","):
         continue
     try:
