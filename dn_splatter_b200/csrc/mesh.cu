@@ -16,7 +16,6 @@
 //           its row's few keys.  No atomics decide any position, so two runs are bit-identical.
 // Workspace: 48 B per grid row in the count phase, 16 B per active cube + 8 B per vertex in the emit phase.
 #include <cub/cub.cuh>
-#include <cuda_fp16.h>
 
 #include "common.cuh"
 #include "mc_tables.cuh"
@@ -32,14 +31,14 @@ struct Cam {
   float E[12];  // world -> camera (OpenCV), row-major [3,4]
 };
 
-__device__ __forceinline__ uint32_t pack_half2(float a, float b) {
-  const __half2 h = __floats2half2_rn(a, b);
-  return *reinterpret_cast<const uint32_t*>(&h);
-}
-__device__ __forceinline__ float2 unpack_half2(uint32_t u) {
-  __half2 h;
-  *reinterpret_cast<uint32_t*>(&h) = u;
-  return __half22float2(h);
+// Voxel colour: the running means of r, g, b as three 21-bit unsigned fixed-point numbers in units of 2^-13 of a level
+// (255 * 2^13 < 2^21), packed r | g << 21 | b << 42 into the 64 bits of q.z (low word) and q.w.  fp16 (0.125-level spacing
+// above 128) rounds away every update smaller than 0.0625 level, so a mean over many views stops following them.
+constexpr int COLOR_FRAC_BITS = 13;
+constexpr uint64_t COLOR_MASK = (1ull << 21) - 1;
+
+__device__ __forceinline__ uint64_t color_bits(const float4& q) {
+  return (uint64_t)__float_as_uint(q.z) | ((uint64_t)__float_as_uint(q.w) << 32);
 }
 
 __global__ void __launch_bounds__(128) tsdf_integrate_kernel(DnrTsdfGrid g, Cam cam, const float* __restrict__ depth,
@@ -69,17 +68,25 @@ __global__ void __launch_bounds__(128) tsdf_integrate_kernel(DnrTsdfGrid g, Cam 
   if (!(sdf > -g.sdf_trunc)) return;
   const float t = fminf(1.f, sdf / g.sdf_trunc);
   // the reference's uint8 colour: np.asarray(rgb * 255, dtype=np.uint8) truncates (clamped here, NaN -> 0)
-  float c[3];
+  int c[3];
 #pragma unroll
-  for (int ch = 0; ch < 3; ++ch) c[ch] = (float)(int)fminf(fmaxf(rgb[3 * pix + ch] * 255.f, 0.f), 255.f);
+  for (int ch = 0; ch < 3; ++ch) c[ch] = (int)fminf(fmaxf(rgb[3 * pix + ch] * 255.f, 0.f), 255.f);
   float4* vox = reinterpret_cast<float4*>(g.voxels) + (((int64_t)i * g.dims[1] + j) * g.dims[2] + k);
-  float4 q = *vox;  // {tsdf, weight, half(r, g), half(b, 0)}
+  float4 q = *vox;  // {tsdf, weight, packed fixed-point r g b}
   const float w = q.y, w1 = w + 1.f;
-  const float2 rg = unpack_half2(__float_as_uint(q.z)), bb = unpack_half2(__float_as_uint(q.w));
+  // colour mean (m * w + c) / (w + 1) in integers, rounded half up; the weight is an integer count (exact below 2^24)
+  const uint64_t wi = (uint64_t)w, den2 = 2 * (wi + 1), cin = color_bits(q);
+  uint64_t cout = 0;
+#pragma unroll
+  for (int ch = 0; ch < 3; ++ch) {
+    const uint64_t m = (cin >> (21 * ch)) & COLOR_MASK;
+    const uint64_t num = m * wi + ((uint64_t)c[ch] << COLOR_FRAC_BITS);
+    cout |= ((2 * num + (wi + 1)) / den2) << (21 * ch);
+  }
   q.x = (q.x * w + t) / w1;
   q.y = w1;
-  q.z = __uint_as_float(pack_half2((rg.x * w + c[0]) / w1, (rg.y * w + c[1]) / w1));
-  q.w = __uint_as_float(pack_half2((bb.x * w + c[2]) / w1, 0.f));
+  q.z = __uint_as_float((uint32_t)cout);
+  q.w = __uint_as_float((uint32_t)(cout >> 32));
   *vox = q;
 }
 
@@ -107,9 +114,10 @@ struct TsdfField {  // 16-byte TSDF voxels: valid where weight > 0
   __device__ __forceinline__ float val(int64_t i) const { return reinterpret_cast<const float2*>(v + i)->x; }
   __device__ __forceinline__ bool ok(int64_t i) const { return reinterpret_cast<const float2*>(v + i)->y > 0.f; }
   __device__ __forceinline__ float3 color(int64_t i) const {
-    const float4 q = v[i];
-    const float2 rg = unpack_half2(__float_as_uint(q.z)), bb = unpack_half2(__float_as_uint(q.w));
-    return make_float3(rg.x, rg.y, bb.x);
+    const uint64_t u = color_bits(v[i]);  // exact in fp32: below 2^21 units
+    constexpr float unit = 1.f / (1 << COLOR_FRAC_BITS);
+    return make_float3((float)(u & COLOR_MASK) * unit, (float)((u >> 21) & COLOR_MASK) * unit,
+                       (float)((u >> 42) & COLOR_MASK) * unit);
   }
 };
 

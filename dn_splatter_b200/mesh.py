@@ -107,7 +107,7 @@ class TSDFVolume:
                              f"{n * VOXEL_BYTES / 2**30:.2f} GiB, over max_bytes = {max_bytes / 2**30:.2f} GiB; use a coarser "
                              "voxel_size or tighter bounds")
         self.voxel_size, self.sdf_trunc, self.depth_trunc = float(voxel_size), float(sdf_trunc), float(depth_trunc)
-        self.voxels = torch.zeros((n, 4), dtype=torch.float32, device=device)  # {tsdf, weight, half rgb + pad}
+        self.voxels = torch.zeros((n, 4), dtype=torch.float32, device=device)  # {tsdf, weight, fixed-point rgb as 64 bits}
         _need_cuda(self.voxels)
         g = self._grid = L.DnrTsdfGrid()
         g.origin[0], g.origin[1], g.origin[2] = self.origin

@@ -347,8 +347,9 @@ int dnr_ray_densities(const float* points, int64_t n_points, const int64_t* nbr_
 
 /* ---- Mesh export (Python surface: dn_splatter_b200.mesh) ----
  * Dense TSDF volume: voxel (i, j, k) is voxels[(i * dims[1] + j) * dims[2] + k] (64-bit index), 16 bytes
- * {float tsdf, float weight, half r, half g, half b, half pad}; colour is the weighted mean of the reference's uint8
- * colours (0..255).  Voxel centres are origin + (index + 0.5) * voxel.  All zero is an empty volume. */
+ * {float tsdf, float weight, uint64 rgb}; colour is the weighted mean of the reference's uint8 colours (0..255), kept as
+ * three 21-bit fixed-point numbers in units of 2^-13 of a level, r | g << 21 | b << 42, rounded half up on each update.
+ * Voxel centres are origin + (index + 0.5) * voxel.  All zero is an empty volume. */
 typedef struct DnrTsdfGrid {
   float origin[3];
   float voxel;     /* voxel edge */

@@ -39,10 +39,10 @@ def _sphere_depth(cam_block, radius=0.5):
 
 
 def _voxels(vol):
-    q = vol.voxels.cpu().numpy()
+    """tsdf, weight and colour (levels, decoded from the voxel's fixed point) of the volume, as [X,Y,Z] grids."""
     shape = tuple(vol.dims)
-    col = q[:, 2:4].copy().view(np.float16)[:, :3]
-    return q[:, 0].reshape(shape), q[:, 1].reshape(shape), col.reshape(shape + (3,))
+    tsdf, w, col = R.unpack_voxels(vol.voxels.cpu().numpy())
+    return tsdf.reshape(shape), w.reshape(shape), col.reshape(shape + (3,))
 
 
 def _views():
@@ -82,7 +82,7 @@ def _integrate_both(bounds=((-0.71, -0.63, -0.77), (0.69, 0.55, 0.83)), voxel=0.
     return vol, (tsdf, w, col), first, first_uv
 
 
-def test_tsdf_integrate_matches_fp32_oracle():
+def test_tsdf_integrate_matches_fp32_oracle_fixed_point_colour():
     vol, (tsdf, w, col), first, (u, v) = _integrate_both()
     assert all(d % 128 for d in vol.dims)
     # after the first view the colour is the pixel the voxel read: (u, v) encoded in red / green
@@ -124,7 +124,7 @@ def test_marching_cubes_matches_oracle_and_is_deterministic():
         np.testing.assert_allclose(got.vertices.cpu().numpy(), rv, rtol=1e-6, atol=1e-7)
 
 
-def test_tsdf_extraction_matches_oracle():
+def test_tsdf_extraction_matches_oracle_fixed_point_colour():
     vol, (tsdf, w, col), _, _ = _integrate_both()
     got = vol.extract_mesh()
     again = vol.extract_mesh()
