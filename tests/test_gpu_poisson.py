@@ -79,20 +79,35 @@ def test_splat_matches_oracle(depth):
 
 
 def test_grid_sample_matches_oracle():
+    """Six point sets, each from the same seed: random points around the grid, points on node centres, points whose
+    floor(x) is the last node (the clamp), an axis with one node, 4 channels, and no points; every grid is also read
+    one channel at a time."""
     from dn_splatter_b200.poisson import grid_sample
 
-    g = np.random.default_rng(2)
-    vals = g.normal(size=(9, 13, 7, 3)).astype(np.float32)
-    origin, cell = (-0.3, 0.2, -1.0), 0.17
-    pts = (np.array(origin) + g.uniform(-0.3, 1.2, (5000, 3)) * np.array([9, 13, 7]) * cell).astype(np.float32)
-    vt, pt = _cuda(vals, pts)
-    for v, w in ((vt, vals), (vt[..., 1].contiguous(), vals[..., 1])):
-        got = grid_sample(v, origin, cell, pt).cpu().numpy()
-        want = P.sample(w, origin, cell, pts)
-        assert np.abs(got - want).max() <= 1e-6 * np.abs(w).max()
+    for case in ("random", "centres", "clamp", "dims1", "channels4", "empty"):
+        g = np.random.default_rng(2)
+        dims = np.array([9, 1, 7] if case == "dims1" else [9, 13, 7])
+        vals = g.normal(size=(*dims, 4 if case == "channels4" else 3)).astype(np.float32)
+        origin, cell = (-0.3, 0.2, -1.0), 0.17
+        n = 0 if case == "empty" else 5000
+        if case == "centres":
+            x = g.integers(0, dims, (n, 3)) + 0.5
+        elif case == "clamp":  # floor(x - 0.5) == dims - 1 on one axis, exactly at the last centre for some
+            x = g.uniform(-0.3, 1.2, (n, 3)) * dims
+            ax = g.integers(0, 3, n)
+            x[np.arange(n), ax] = dims[ax] - 0.5 + np.where(np.arange(n) % 4 == 0, 0.0, g.uniform(0, 1, n))
+        else:
+            x = g.uniform(-0.3, 1.2, (n, 3)) * dims
+        pts = (np.array(origin) + x * cell).astype(np.float32)
+        vt, pt = _cuda(vals, pts)
+        for v, w in ((vt, vals), (vt[..., 1].contiguous(), vals[..., 1])):
+            got = grid_sample(v, origin, cell, pt).cpu().numpy()
+            assert got.shape == (n,) + w.shape[3:], case
+            want = P.sample(w, origin, cell, pts)
+            assert np.abs(got - want).max(initial=0.0) <= 1e-6 * np.abs(w).max(), case
 
 
-@pytest.mark.parametrize("depth", [5, 6])
+@pytest.mark.parametrize("depth", [4, 5, 6])
 @pytest.mark.parametrize("alpha", [0.0, 4.0])
 def test_multigrid_matches_direct_solve(depth, alpha):
     from dn_splatter_b200.poisson import poisson_grid, poisson_solve, poisson_splat
