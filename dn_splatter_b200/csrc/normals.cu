@@ -23,7 +23,8 @@
 //      key exceeds the running k-th key are dropped, and the shared-memory buffer is cut back to its k best by a
 //      weighted radix select whenever it fills.
 // The cell of a coordinate is floor((x - lo) / cell) clamped to the grid, a monotone function of x, so a point within
-// R of the query along every axis lies in a visited cell (R carries a 2^-40 relative margin over the rounded distance).
+// R of the query along every axis lies in a visited cell (R carries a 2^-40 relative margin over the rounded distance and
+// is at least 2^-510, which covers squared distances that underflowed).
 // Work per query therefore depends on the local density only, not on how many points coincide.
 #include <cub/cub.cuh>
 
@@ -404,7 +405,9 @@ __global__ void __launch_bounds__(32 * QWARPS) nrm_query_kernel(QueryArgs a) {
       uint32_t rem;
       Key t = weighted_select(b, cnt, kk, rem);
       cnt = compact(b, cnt, t);
-      const double R = sqrt(__longlong_as_double((long long)t.hi)) * (1.0 + 0x1p-40);
+      // the floor: a d2 below 2^-1022 carries an absolute rounding error (dx * dx may underflow to 0), so the true
+      // distance is only known to lie below 2^-511
+      const double R = fmax(sqrt(__longlong_as_double((long long)t.hi)) * (1.0 + 0x1p-40), 0x1p-510);
       int level = 0;
       while (level < MORTON_BITS && a.cell * (double)(1 << level) * LEVEL_DIV < R) ++level;
       uint32_t c0[3], c1[3];

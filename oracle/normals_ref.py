@@ -65,13 +65,290 @@ def knn(points: np.ndarray, k: int, queries=None):
         if u not in cache:
             d2 = sq_dist(uniq[u], uniq)
             order = np.lexsort((first, d2))
-            c = np.cumsum(counts[order])
-            last = int(np.searchsorted(c, kk))
-            take = counts[order[: last + 1]].copy()
-            take[-1] -= c[last] - kk
-            cache[u] = np.repeat(first[order[: last + 1]], take)
+            cache[u] = _cut(first[order], counts[order], kk)
         out.append(cache[u])
     return out
+
+
+def _cut(order_first, order_counts, kk, split=True):
+    """The neighbour list of positions already in key order: copies until kk, the last position's split."""
+    c = np.cumsum(order_counts)
+    last = int(np.searchsorted(c, kk))
+    take = order_counts[: last + 1].copy()
+    if split:
+        take[-1] -= c[last] - kk
+    return np.repeat(order_first[: last + 1], take)
+
+
+def knn_fast(points: np.ndarray, k: int, queries):
+    """knn(points, k, queries) under the same tie rule, fast at millions of points: the min(kk, U) nearest positions of a
+    cKDTree give the kk-th squared distance; a ball query at a slightly inflated radius (the tree rounds its own
+    distances) closes the set, whose d2 are recomputed exactly, ordered by (d2, smallest index) and cut at kk."""
+    from scipy.spatial import cKDTree
+
+    uniq, first, counts, inv = unique_positions(points)
+    kk = min(k, len(points))
+    qu = inv[np.asarray(queries, np.int64)]
+    us, back = np.unique(qu, return_inverse=True)
+    tree = cKDTree(uniq)
+    m = min(kk, len(uniq))
+    _, idx = tree.query(uniq[us], k=m, workers=-1)
+    idx = idx.reshape(len(us), m)
+    d2 = sq_dist(uniq[us][:, None, :], uniq[idx])
+    o = np.lexsort((first[idx], d2), axis=-1)
+    d2s = np.take_along_axis(d2, o, 1)
+    cum = np.cumsum(np.take_along_axis(counts[idx], o, 1), axis=1)
+    kth = d2s[np.arange(len(us)), np.argmax(cum >= kk, axis=1)]
+    balls = tree.query_ball_point(uniq[us], np.sqrt(kth) * (1 + 2.0 ** -20) + 2.0 ** -500, workers=-1)
+    res = []
+    for i, b in enumerate(balls):
+        b = np.asarray(b, np.int64)
+        e = sq_dist(uniq[us[i]], uniq[b])
+        oo = np.lexsort((first[b], e))
+        assert counts[b].sum() >= kk
+        res.append(_cut(first[b][oo], counts[b][oo], kk))
+    return [res[j] for j in back]
+
+
+# ---- numpy restatement of dnr_dn_normals' search geometry (csrc/normals.cu) ----
+MORTON_BITS = 21
+CAP = 768  # candidate buffer entries per warp; the kernel compacts before a 32-entry push batch when more than CAP - 32
+R_MARGIN = 1.0 + 2.0 ** -40
+R_FLOOR = 2.0 ** -510  # a k-th d2 that underflowed below 2^-1022 says only that the true distance is below 2^-511
+
+# Plausible kernel mistakes; search_mirror(..., slip=...) restates each (tests/test_normals_search_cpu.py shows every one
+# changes some query's neighbour multiset or examined count on the GPU test's cases).
+SEARCH_SLIPS = {
+    "no_margin": "R is the rounded k-th distance, without the 2^-40 relative margin",
+    "no_floor": "R is not floored, so a k-th d2 that underflowed to 0 or a subnormal gives a box of one cell",
+    "cell_unclamped": "cell_of clamps at 0 (the u32 conversion saturates) but not at 2^21 - 1",
+    "unweighted": "the selects count positions instead of points (multiplicities ignored)",
+    "largest_index": "among equal squared distances the largest smallest-index wins",
+    "no_split": "the k-th position contributes all its copies (rem ignored)",
+    "window_twice": "window entries are pushed again when a cell range covers them",
+}
+
+
+def grid_of(points: np.ndarray):
+    """(lo [3], cell) as estimate_normals sets them: the bounding box's low corner and its largest extent / 2^21."""
+    p = np.asarray(points, np.float64)
+    lo, hi = p.min(0), p.max(0)
+    extent = float((hi - lo).max())
+    return lo, (extent / (1 << MORTON_BITS) if extent > 0 else 1.0)
+
+
+def _spread3(v):
+    x = v.astype(np.uint64) & np.uint64(0x1FFFFF)
+    for s, m in ((32, 0x1F00000000FFFF), (16, 0x1F0000FF0000FF), (8, 0x100F00F00F00F00F), (4, 0x10C30C30C30C30C3),
+                 (2, 0x1249249249249249)):
+        x = (x | (x << np.uint64(s))) & np.uint64(m)
+    return x
+
+
+def morton(cx, cy, cz):
+    return _spread3(cx) | (_spread3(cy) << np.uint64(1)) | (_spread3(cz) << np.uint64(2))
+
+
+def _floor_cell(x, lo, inv):
+    return np.floor((x - lo) * inv)
+
+
+def cell_of(x, lo, inv, clamp=True):
+    c = np.maximum(_floor_cell(x, lo, inv), 0.0)
+    if clamp:
+        c = np.minimum(c, float((1 << MORTON_BITS) - 1))
+    return c.astype(np.uint64)
+
+
+def search_order(points: np.ndarray, lo, cell, slip=None):
+    """The kernel's distinct positions in its order (Morton key, then x / y / z bits, then index, all stable):
+    (upts [U,3], ukey [U] u64, umin [U], count [U], position of each point [N])."""
+    p = np.asarray(points, np.float64) + 0.0
+    inv = 1.0 / cell
+    cl = slip != "cell_unclamped"
+    key = morton(*(cell_of(p[:, a], lo[a], inv, cl) for a in range(3)))
+    bits = p.view(np.uint64)
+    order = np.lexsort((bits[:, 2], bits[:, 1], bits[:, 0], key))
+    ps = p[order]
+    head = np.r_[True, (ps[1:] != ps[:-1]).any(1)]
+    ustart = np.flatnonzero(head)
+    count = np.diff(np.r_[ustart, len(p)])
+    pos = np.empty(len(p), np.int64)
+    pos[order] = np.cumsum(head) - 1
+    return ps[ustart], key[order[ustart]], order[ustart], count, pos
+
+
+def _le(d2, tie, td2, ttie):
+    return (d2 < td2) | ((d2 == td2) & (tie <= ttie))
+
+
+def _kth(d2, tie, w, kk):
+    """(d2, tie) of the kk-th point by weight in (d2, tie) order, over one row (1-D arrays)."""
+    o = np.lexsort((tie, d2))
+    i = int(np.argmax(np.cumsum(w[o]) >= kk))
+    return d2[o[i]], tie[o[i]]
+
+
+def search_mirror(points: np.ndarray, k: int, queries, lo=None, cell=None, slip=None, chunk_entries=1 << 23):
+    """The search of dnr_dn_normals restated per query point.  Returns a dict of per-query arrays:
+    nbrs (the neighbour multiset's smallest indices, in (d2, index) order), examined (the window's size plus the sizes of
+    every scanned cell range, as the kernel counts them), shortcut (multiplicity >= kk), everything (the window is every
+    position), level (-1 without a grid search), level_clamped (the level rule reached 21: R above the extent, one cell),
+    box_clamped (the
+    box [q - R, q + R] left the grid on some axis), compactions (mid-scan buffer compactions: the kernel's pushes
+    simulated in their 32-entry batches)."""
+    assert slip is None or slip in SEARCH_SLIPS, slip
+    pts = np.asarray(points, np.float64)
+    n = len(pts)
+    if lo is None:
+        lo, cell = grid_of(pts)
+    lo = np.asarray(lo, np.float64)
+    inv = 1.0 / cell
+    kk = min(k, n)
+    upts, ukey, umin, count, pos = search_order(pts, lo, cell, slip)
+    U = len(upts)
+    tie_of = (lambda f: -f.astype(np.int64)) if slip == "largest_index" else (lambda f: f.astype(np.int64))
+    utie = tie_of(umin)
+    wsel = np.ones(U, np.int64) if slip == "unweighted" else count.astype(np.int64)
+    qu_all = pos[np.asarray(queries, np.int64)]
+    us, back = np.unique(qu_all, return_inverse=True)
+    nq = len(us)
+    out = dict(examined=np.zeros(nq, np.int64), R=np.zeros(nq), split=np.zeros(nq, bool), shortcut=count[us] >= kk,
+               everything=np.zeros(nq, bool),
+               level=np.full(nq, -1), level_clamped=np.zeros(nq, bool), box_clamped=np.zeros(nq, bool),
+               compactions=np.zeros(nq, np.int64))
+    nbrs = [None] * nq
+    # R: the search radius of a grid search; split: the kk-th point is one of several copies of its position
+
+    def finish(i, d2, tie, w_cut, ucand):
+        o = np.lexsort((tie, d2))
+        f = umin[ucand[o]]
+        if slip == "unweighted":  # the kk-th position by count; every copy of the earlier ones, rem = 1 for the last
+            m = min(kk, len(o))
+            nbrs[i] = np.r_[np.repeat(f[: m - 1], count[ucand[o[: m - 1]]]), f[m - 1: m]][:k] if m else f[:0]
+        else:
+            nbrs[i] = _cut(f, w_cut[o], kk, split=slip != "no_split")
+        out["split"][i] = np.searchsorted(np.cumsum(w_cut[o]), kk) < len(o) and np.cumsum(w_cut[o])[
+            np.searchsorted(np.cumsum(w_cut[o]), kk)] > kk
+
+    for i in np.flatnonzero(out["shortcut"]):
+        nbrs[i] = _cut(umin[us[i]: us[i] + 1], count[us[i]: us[i] + 1], kk, split=slip != "no_split")
+        out["split"][i] = count[us[i]] > kk
+    rest = np.flatnonzero(~out["shortcut"])
+    win = np.arange(-kk, kk + 1)
+    # queries in chunks bounded by the window entries (cell ranges are split further below)
+    step = max(1, chunk_entries // (8 * (2 * kk + 1)))
+    for c0 in range(0, len(rest), step):
+        rows = rest[c0: c0 + step]
+        u = us[rows]
+        wlo, whi = np.maximum(u - kk, 0), np.minimum(u + kk + 1, U)
+        j = u[:, None] + win[None, :]
+        ok = (j >= wlo[:, None]) & (j < whi[:, None])
+        jc = np.clip(j, 0, U - 1)
+        q = upts[u]
+        wd2 = np.where(ok, sq_dist(q[:, None, :], upts[jc]), np.inf)
+        wtie = np.where(ok, utie[jc], np.iinfo(np.int64).max)
+        ww = np.where(ok, wsel[jc], 0)
+        out["examined"][rows] = whi - wlo
+        every = (wlo == 0) & (whi == U)
+        out["everything"][rows] = every
+        o = np.lexsort((wtie, wd2), axis=-1)
+        cum = np.cumsum(np.take_along_axis(ww, o, 1), axis=1)
+        at = np.take_along_axis(o, np.argmax(cum >= kk, axis=1)[:, None], 1)[:, 0]
+        td2 = wd2[np.arange(len(rows)), at]
+        ttie = wtie[np.arange(len(rows)), at]
+        R = np.sqrt(td2) * (1.0 if slip == "no_margin" else R_MARGIN)
+        if slip != "no_floor":
+            R = np.maximum(R, R_FLOOR)
+        level = np.zeros(len(rows), np.int64)
+        for l in range(MORTON_BITS):
+            level += cell * float(1 << l) * 2 < R
+        lclamp = level == MORTON_BITS
+        cl = slip != "cell_unclamped"
+        c_lo = np.stack([cell_of(q[:, a] - R, lo[a], inv, cl) for a in range(3)], 1) >> level[:, None].astype(np.uint64)
+        c_hi = np.stack([cell_of(q[:, a] + R, lo[a], inv, cl) for a in range(3)], 1) >> level[:, None].astype(np.uint64)
+        top = float((1 << MORTON_BITS) - 1)
+        bclamp = ((_floor_cell(q - R[:, None], lo, inv) < 0) | (_floor_cell(q + R[:, None], lo, inv) > top)).any(1)
+        nxyz = (c_hi.astype(np.int64) - c_lo.astype(np.int64) + 1)
+        ncell = np.where(every, 0, nxyz.prod(1))
+        grid = ~every
+        out["level"][rows[grid]] = level[grid]
+        out["R"][rows[grid]] = R[grid]
+        out["level_clamped"][rows] = lclamp & grid
+        out["box_clamped"][rows] = bclamp & grid
+        mc = int(ncell.max()) if len(ncell) else 0
+        cidx = np.arange(mc)[None, :]
+        cvalid = cidx < ncell[:, None]
+        nx, ny = nxyz[:, :1], nxyz[:, 1:2]
+        cx = c_lo[:, :1].astype(np.int64) + cidx % nx
+        cy = c_lo[:, 1:2].astype(np.int64) + (cidx // nx) % ny
+        cz = c_lo[:, 2:3].astype(np.int64) + cidx // (nx * ny)
+        sh = level[:, None].astype(np.uint64)
+        k0 = morton(np.where(cvalid, cx, 0).astype(np.uint64) << sh, np.where(cvalid, cy, 0).astype(np.uint64) << sh,
+                    np.where(cvalid, cz, 0).astype(np.uint64) << sh)
+        s = np.searchsorted(ukey, k0, "left")
+        e = np.searchsorted(ukey, k0 + (np.uint64(1) << (np.uint64(3) * sh)), "left")
+        ln = np.where(cvalid, e - s, 0)
+        out["examined"][rows] += ln.sum(1)
+        # candidates, query by query in sub-chunks bounded by their entries
+        tot = ln.sum(1)
+        r0 = 0
+        while r0 < len(rows):
+            r1 = r0 + max(1, int(np.searchsorted(np.cumsum(tot[r0:]), chunk_entries, "right")))
+            sl = slice(r0, r1)
+            L = ln[sl].reshape(-1)
+            starts = s[sl].reshape(-1)
+            cid = np.repeat(np.arange(L.size), L)
+            off = np.arange(L.sum()) - np.repeat(np.cumsum(L) - L, L)
+            jj = starts[cid] + off
+            qi = cid // mc
+            inwin = (jj >= wlo[sl][qi]) & (jj < whi[sl][qi])
+            d2 = sq_dist(q[sl][qi], upts[jj])
+            keep = _le(d2, utie[jj], td2[sl][qi], ttie[sl][qi]) & ((~inwin) | (slip == "window_twice"))
+            qs = np.searchsorted(qi, np.arange(r1 - r0 + 1))  # the entries of each query are contiguous
+            # mid-scan compactions, where the pushes could overflow the buffer
+            wkeep = _le(wd2[sl], wtie[sl], td2[sl, None], ttie[sl, None]) & ok[sl]
+            bound = wkeep.sum(1) + np.bincount(qi[keep], minlength=r1 - r0)
+            for b in np.flatnonzero((bound > CAP - 32) & grid[sl]):
+                m = slice(qs[b], qs[b + 1])
+                bb = np.cumsum(np.r_[0, -(-L[b * mc: (b + 1) * mc] // 32)])  # first batch ordinal of each cell
+                batch = bb[cid[m] - b * mc] + off[m] // 32
+                out["compactions"][rows[r0 + b]] = _compactions(
+                    wd2[r0 + b][wkeep[b]], wtie[r0 + b][wkeep[b]], ww[r0 + b][wkeep[b]], d2[m], utie[jj[m]], wsel[jj[m]],
+                    batch, keep[m], int(bb[-1]), td2[r0 + b], ttie[r0 + b], kk)
+            for b in range(r1 - r0):
+                m = slice(qs[b], qs[b + 1])
+                km = keep[m]
+                wm = ok[r0 + b]
+                ucand = np.r_[j[r0 + b][wm], jj[m][km]]
+                finish(rows[r0 + b], np.r_[wd2[r0 + b][wm], d2[m][km]], np.r_[wtie[r0 + b][wm], utie[jj[m][km]]],
+                       count[ucand].astype(np.int64), ucand)
+            r0 = r1
+    out = {key: v[back] for key, v in out.items()}
+    out["nbrs"] = [nbrs[b] for b in back]
+    return out
+
+
+def _compactions(bd2, btie, bw, d2, tie, w, batch, pushable, nbatch, td2, ttie, kk):
+    """How many times the kernel's buffer is cut back mid-scan: before each 32-entry batch (nbatch of them) it compacts
+    when it holds more than CAP - 32 entries; a batch pushes its entries whose key is <= the running k-th key."""
+    cnt, comps, b0 = len(bd2), 0, 0
+    buf = [bd2, btie, bw]
+    d2, tie, w, batch = d2[pushable], tie[pushable], w[pushable], batch[pushable]
+    while True:
+        live = (batch >= b0) & _le(d2, tie, td2, ttie)
+        per = np.bincount(batch[live] - b0, minlength=nbatch - b0)
+        before = cnt + np.r_[0, np.cumsum(per)[:-1]]
+        over = np.flatnonzero(before > CAP - 32)
+        if not len(over):
+            return comps
+        b = b0 + int(over[0])
+        took = live & (batch < b)
+        buf = [np.r_[buf[0], d2[took]], np.r_[buf[1], tie[took]], np.r_[buf[2], w[took]]]
+        td2, ttie = _kth(buf[0], buf[1], buf[2], kk)
+        kept = _le(buf[0], buf[1], td2, ttie)
+        buf = [a[kept] for a in buf]
+        cnt, comps, b0 = len(buf[0]), comps + 1, b
 
 
 def covariance(points: np.ndarray, nbr: np.ndarray) -> np.ndarray:
