@@ -30,6 +30,8 @@ constexpr int BOX_THREADS = 256;
 constexpr int RASTER_THREADS = 256;
 constexpr int VIS_THREADS = 128;
 
+// Workspace of dnr_mesh_depth.  tests/test_gpu_mesh_eval_kernels.py reads the last view's boxes, counts and scan back
+// from it at these offsets (int4 boxes at 0, then the int64 arrays at 256-B boundaries): change both together.
 struct DepthLayout {
   size_t boxes, counts, scan, cub_temp, total, cub_bytes;
 };

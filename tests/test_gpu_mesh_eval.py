@@ -8,6 +8,8 @@ import pytest
 import torch
 
 from oracle import mesh_eval_ref as R
+from tests import mesh_eval_cases as C
+from tests.mesh_eval_cases import box, sphere
 
 pytestmark = [pytest.mark.gpu,
               pytest.mark.skipif(not torch.cuda.is_available(), reason="needs a CUDA device")]
@@ -38,115 +40,59 @@ def _mesh(v, f):
     return TriangleMesh(torch.as_tensor(np.asarray(v), dtype=torch.float32), torch.as_tensor(np.asarray(f), dtype=torch.int32), None)
 
 
-def box(lo=(-1.0, -1.0, -1.0), hi=(1.0, 1.0, 1.0)):
-    lo, hi = np.asarray(lo, np.float64), np.asarray(hi, np.float64)
-    v = np.array([[hi[0] if i & 1 else lo[0], hi[1] if i & 2 else lo[1], hi[2] if i & 4 else lo[2]] for i in range(8)])
-    f = np.array([[0, 2, 1], [1, 2, 3], [4, 5, 6], [5, 7, 6], [0, 1, 4], [1, 5, 4], [2, 6, 3], [3, 6, 7],
-                  [0, 4, 2], [2, 4, 6], [1, 3, 5], [3, 7, 5]])
-    return v, f
-
-
-def sphere(n=16, r=0.6, c=(0.0, 0.0, 0.0)):
-    th, ph = np.meshgrid(np.linspace(0, np.pi, n + 1), np.linspace(0, 2 * np.pi, 2 * n + 1), indexing="ij")
-    v = np.stack([np.sin(th) * np.cos(ph), np.sin(th) * np.sin(ph), np.cos(th)], -1).reshape(-1, 3) * r + np.asarray(c)
-    idx = np.arange(v.shape[0]).reshape(n + 1, 2 * n + 1)
-    a, b, cc, d = idx[:-1, :-1], idx[:-1, 1:], idx[1:, :-1], idx[1:, 1:]
-    return v, np.concatenate([np.stack([a, cc, b], -1).reshape(-1, 3), np.stack([b, cc, d], -1).reshape(-1, 3)])
-
-
-def odd_triangles():
-    """Seen from an identity OpenGL camera (looking down -z): triangles straddling the near plane, beyond far, behind the
-    camera, back-facing, full-screen, sub-pixel and degenerate."""
-    tris = [
-        [[-0.5, -0.4, -0.005], [0.6, -0.3, -3.0], [0.1, 0.7, -2.5]],      # straddles near = 0.01
-        [[-0.3, -0.3, -12.0], [0.3, -0.3, -12.0], [0.0, 0.3, -12.0]],     # beyond far
-        [[-0.3, -0.3, -9.0], [0.3, -0.3, -11.0], [0.0, 0.3, -9.5]],       # straddles far
-        [[-0.5, -0.5, 2.0], [0.5, -0.5, 2.0], [0.0, 0.5, 2.0]],           # behind the camera
-        [[0.2, 0.1, -1.5], [0.1, 0.4, -1.5], [0.4, 0.3, -1.6]],           # back-facing winding
-        [[-40.0, -40.0, -6.0], [40.0, -40.0, -6.5], [0.0, 60.0, -6.2]],   # full screen
-        [[0.0101, 0.0102, -1.0], [0.0104, 0.0101, -1.0], [0.0102, 0.0105, -1.0]],  # sub-pixel
-        [[0.1, 0.1, -2.0], [0.2, 0.2, -2.0], [0.3, 0.3, -2.0]],           # degenerate (collinear)
-        [[-0.2, 0.0, -1.0], [-0.2, 0.0, -1.0], [-0.1, 0.2, -1.0]],        # degenerate (repeated vertex)
-        [[-0.9, -0.9, -3.0], [-0.1, -0.8, -0.5], [-0.5, 0.2, 3.0]],       # reaches behind the camera
-    ]
-    v = np.asarray(tris, np.float64).reshape(-1, 3)
-    return v, np.arange(v.shape[0]).reshape(-1, 3)
-
-
-def edge_grid(W, H, f):
-    """A triangulated grid at z = -2 whose vertices project exactly onto pixel centres, so its edges pass through them."""
-    cx, cy = W / 2, H / 2
-    xs = ((np.arange(2, W - 2, 3) + 0.5 - cx) / f) * 2.0
-    ys = ((np.arange(2, H - 2, 3) + 0.5 - cy) / f) * 2.0
-    X, Y = np.meshgrid(xs, ys)
-    v = np.stack([X.reshape(-1), -Y.reshape(-1), np.full(X.size, -2.0)], 1)  # image y points down, world y up
-    nx = xs.shape[0]
-    idx = np.arange(v.shape[0]).reshape(ys.shape[0], nx)
-    a, b, c, d = idx[:-1, :-1], idx[:-1, 1:], idx[1:, :-1], idx[1:, 1:]
-    fl = np.concatenate([np.stack([a, c, b], -1).reshape(-1, 3), np.stack([b, c, d], -1).reshape(-1, 3)])
-    return v, fl
-
-
 def _scenes(W, H):
-    eye = np.eye(4)[:3]
-    out = [("box_inside", *box(), _cam(_look_at((0.1, -0.2, 0.05), (1.0, 0.3, 0.2)), W, H, 0.6 * W)),
-           ("sphere", *sphere(), _cam(_look_at((0.3, -2.0, 0.4), (0.0, 0.0, 0.0)), W, H, 1.1 * W, 1.0 * W, W / 2 - 1.3, H / 2 + 0.7)),
-           ("odd", *odd_triangles(), _cam(eye, W, H, 0.8 * W))]
-    gv, gf = edge_grid(W, H, 0.7 * W)
-    out.append(("edges", gv, gf, _cam(eye, W, H, 0.7 * W)))
-    return out
+    return [(name, v, f, _cam(c2w, W, H, fx, fy, cx, cy)) for name, v, f, c2w, fx, fy, cx, cy in C.legacy_scenes(W, H)]
 
 
 def _compare_depth(name, v, f, cam, W, H, chunk=64):
-    from dn_splatter_b200.mesh_eval import render_mesh_depth
+    """The kernel's depth against the oracle's restatement of its rule on the fp32 camera block it reads: every pixel's
+    bits equal.  The independent ray cast (fp64 Moller-Trumbore) agrees on hits away from triangle edges, to 1 fp32 ulp.
+    Returns (kernel depth, ray-cast depth, near-edge pixel count, the rule's decision counts)."""
+    from dn_splatter_b200.mesh_eval import camera_blocks, render_mesh_depth
 
     got = render_mesh_depth(_mesh(v, f), [cam])[0]
     again = render_mesh_depth(_mesh(v, f), [cam])[0]
     assert torch.equal(got, again), name
     got = got.cpu().numpy()
-    blk = _block(cam)
-    v32 = np.asarray(v, np.float32).astype(np.float64)  # the kernel reads float32 vertices
-    want = R.ray_cast_depth(v32, f, blk, W, H, chunk=chunk)
-    amb = R.near_edge_pixels(v32, f, blk, W, H, chunk=chunk)
-    differ = (got > 0) != (want > 0)
-    assert not (differ & ~amb).any(), (name, int((differ & ~amb).sum()))
-    both = (got > 0) & (want > 0) & ~amb
-    rel = np.abs(got[both] - want[both]) / want[both]
-    assert rel.max() <= 1e-5, (name, float(rel.max()))
-    return got, want, int(amb.sum()), int(differ.sum())
+    blk = camera_blocks([cam], torch.float32).cpu().numpy()[0]
+    assert np.array_equal(blk, _block(cam).astype(np.float32)), name
+    v32 = np.asarray(v, np.float32)  # the kernel reads float32 vertices
+    want, stats = R.depth_kernel_rule(v32, f, blk, W, H)
+    n_diff = int((got.view(np.uint32) != want.view(np.uint32)).sum())
+    assert n_diff == 0, (name, n_diff)
+    rc = R.ray_cast_depth(v32.astype(np.float64), f, blk.astype(np.float64), W, H, chunk=chunk)
+    amb = R.near_edge_pixels(v32.astype(np.float64), f, blk.astype(np.float64), W, H, chunk=chunk)
+    assert np.array_equal((got > 0)[~amb], (rc > 0)[~amb]), name
+    both = (got > 0) & (rc > 0) & ~amb
+    ulp = np.abs(got[both].view(np.int32).astype(np.int64) - rc[both].astype(np.float32).view(np.int32).astype(np.int64))
+    assert ulp.max(initial=0) <= 1, (name, int(ulp.max()))
+    return got, rc, int(amb.sum()), stats
 
 
 @pytest.mark.parametrize("W,H", [(81, 49), (75, 53)])
 def test_mesh_depth_matches_the_oracle_ray_cast(W, H):
     report = {}
     for name, v, f, cam in _scenes(W, H):
-        got, want, n_amb, n_diff = _compare_depth(name, v, f, cam, W, H)
-        report[name] = (n_amb, n_diff)
-        assert n_diff <= max(4, 0.01 * W * H), (name, n_diff)
+        got, rc, n_amb, stats = _compare_depth(name, v, f, cam, W, H)
+        report[name] = (n_amb, stats)
         if name == "box_inside":
             assert (got > 0).all()  # a closed box seen from inside has no empty pixel
         if name == "edges":
-            hit = want > 0
-            inner = hit.copy()  # hit pixels whose 4 neighbours are hit: away from the grid's outer boundary
-            inner[1:-1, 1:-1] &= hit[:-2, 1:-1] & hit[2:, 1:-1] & hit[1:-1, :-2] & hit[1:-1, 2:]
-            inner[[0, -1], :] = False
-            inner[:, [0, -1]] = False
+            # pixels the independent ray cast hits along with their 4 neighbours: away from the grid's outer boundary
+            inner = C.interior_hits(v, f, _block(cam).astype(np.float32), W, H)
             assert inner.sum() > 0.5 * W * H and (got[inner] > 0).all()  # no pixel centre on a shared edge is lost
         if name == "odd":
             assert (got > 0).all() and (got < 5.0).any()  # the full-screen triangle behind the nearer ones
-    print("near-edge pixels / differing hit pixels", report)
+    print("near-edge pixels / pixels per decision of the rule", report)
 
 
 def test_mesh_depth_full_hd():
     W, H = 1920, 1080
-    v1, f1 = odd_triangles()
-    v2, f2 = box((-3.0, -3.0, -8.0), (3.0, 3.0, 1.0))
-    v = np.concatenate([v1, v2])
-    f = np.concatenate([f1, f2 + v1.shape[0]])
-    cam = _cam(np.eye(4)[:3], W, H, 1100.0, 1090.0, 961.3, 538.9)
-    got, want, n_amb, n_diff = _compare_depth("full_hd", v, f, cam, W, H, chunk=2)
-    assert (got > 0).mean() > 0.99 and n_diff <= 50
-    print("1080p near-edge pixels", n_amb, "differing", n_diff)
+    v, f, c2w, fx, fy, cx, cy = C.full_hd_scene()
+    cam = _cam(c2w, W, H, fx, fy, cx, cy)
+    got, rc, n_amb, stats = _compare_depth("full_hd", v, f, cam, W, H, chunk=2)
+    assert (got > 0).mean() > 0.99
+    print("1080p near-edge pixels", n_amb, "pixels per decision", stats)
 
 
 def test_mesh_depth_batches_views():
