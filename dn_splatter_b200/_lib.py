@@ -369,3 +369,33 @@ def check(code: int, what: str) -> None:
     if code != 0:
         msg = load().dnr_error_string(code).decode()
         raise DnrError(f"{what} failed with code {code}: {msg}")
+
+
+def stream() -> C.c_void_p:
+    """The current CUDA stream, as the `void* stream` argument of a library call."""
+    import torch
+
+    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
+
+
+def need_cuda(*tensors) -> None:
+    for t in tensors:
+        if t.device.type != "cuda":
+            raise DnrError("dn_splatter_b200 needs CUDA tensors (no CPU path)")
+
+
+def workspace_bytes(query, *args) -> int:
+    """What the `dnr_*_workspace_bytes` query asks for; raises with the library's error code when it returns one."""
+    n = int(query(*args))
+    if n < 0:
+        check(n, query.__name__)
+    return n
+
+
+def workspace(query, *args, device):
+    """(uint8 workspace on `device`, its size in bytes) for the `dnr_*_workspace_bytes` query.  At least one byte is
+    allocated: a zero-byte tensor's data_ptr() is 0, which the library rejects as DNR_E_NULL."""
+    import torch
+
+    n = workspace_bytes(query, *args)
+    return torch.empty(max(n, 1), dtype=torch.uint8, device=device), n

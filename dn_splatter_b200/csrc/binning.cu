@@ -29,8 +29,6 @@
 
 namespace {
 
-inline size_t align_up(size_t x, size_t a = 256) { return (x + a - 1) / a * a; }
-
 struct ToI64 {
   __host__ __device__ __forceinline__ int64_t operator()(int32_t v) const { return (int64_t)v; }
 };
@@ -41,6 +39,7 @@ __global__ void iota_kernel(int32_t* out, int32_t n) {
 }
 
 struct ScanWs {
+  DnrCarver carve;
   uint32_t* keys_sorted;
   int32_t* order;
   int32_t* iota;
@@ -48,28 +47,21 @@ struct ScanWs {
   int64_t* isect_start;  // [N+1]
   void* cub_temp;
   size_t cub_bytes;
-  size_t total;
+  ScanWs(void* base, int32_t n) : carve(base) {
+    keys_sorted = carve.take<uint32_t>(n);
+    order = carve.take<int32_t>(n);
+    iota = carve.take<int32_t>(n);
+    counts = carve.take<int32_t>((size_t)n + 1);
+    isect_start = carve.take<int64_t>((size_t)n + 1);
+    size_t sort_bytes = 0, scan_bytes = 0;
+    const cudaError_t e1 = cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                                           (const int32_t*)nullptr, (int32_t*)nullptr, n, 0, 32);
+    auto it = thrust::make_transform_iterator((const int32_t*)nullptr, ToI64());
+    const cudaError_t e2 = cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, it, (int64_t*)nullptr, n + 1);
+    cub_bytes = sort_bytes > scan_bytes ? sort_bytes : scan_bytes;
+    cub_temp = carve.cub_scratch(e1 != cudaSuccess ? e1 : e2, cub_bytes);
+  }
 };
-
-ScanWs carve_scan(void* base, int32_t n) {
-  ScanWs w;
-  size_t off = 0;
-  char* p = (char*)base;
-  w.keys_sorted = (uint32_t*)(p + off); off += align_up((size_t)n * 4);
-  w.order = (int32_t*)(p + off); off += align_up((size_t)n * 4);
-  w.iota = (int32_t*)(p + off); off += align_up((size_t)n * 4);
-  w.counts = (int32_t*)(p + off); off += align_up((size_t)(n + 1) * 4);
-  w.isect_start = (int64_t*)(p + off); off += align_up((size_t)(n + 1) * 8);
-  size_t sort_bytes = 0, scan_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
-                                  (int32_t*)nullptr, n, 0, 32);
-  auto it = thrust::make_transform_iterator((const int32_t*)nullptr, ToI64());
-  cub::DeviceScan::ExclusiveSum(nullptr, scan_bytes, it, (int64_t*)nullptr, n + 1);
-  w.cub_bytes = sort_bytes > scan_bytes ? sort_bytes : scan_bytes;
-  w.cub_temp = (void*)(p + off); off += align_up(w.cub_bytes);
-  w.total = off;
-  return w;
-}
 
 // the padding key is n_tiles (one past the last list id), so `tile_bits` = bits of the value n_tiles
 template <typename KeyT>
@@ -80,31 +72,22 @@ inline int sort_end_bit(int tile_bits) {
 
 template <typename KeyT>
 struct SortWs {
+  DnrCarver carve;
   KeyT* keys_in;
   KeyT* keys_out;
   int32_t* gids_in;
   void* cub_temp;
-  size_t cub_bytes;
-  size_t total;
+  size_t cub_bytes = 0;
+  SortWs(void* base, int64_t n_isects, int tile_bits) : carve(base) {
+    const size_t n = (size_t)(n_isects > 0 ? n_isects : 1);
+    keys_in = carve.template take<KeyT>(n);
+    keys_out = carve.template take<KeyT>(n);
+    gids_in = carve.template take<int32_t>(n);
+    const cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const KeyT*)nullptr, (KeyT*)nullptr, (const int32_t*)nullptr,
+                                                          (int32_t*)nullptr, (int64_t)n, 0, sort_end_bit<KeyT>(tile_bits));
+    cub_temp = carve.cub_scratch(e, cub_bytes);
+  }
 };
-
-template <typename KeyT>
-SortWs<KeyT> carve_sort(void* base, int64_t n_isects, int tile_bits) {
-  SortWs<KeyT> w;
-  size_t off = 0;
-  char* p = (char*)base;
-  const size_t n = (size_t)(n_isects > 0 ? n_isects : 1);
-  w.keys_in = (KeyT*)(p + off); off += align_up(n * sizeof(KeyT));
-  w.keys_out = (KeyT*)(p + off); off += align_up(n * sizeof(KeyT));
-  w.gids_in = (int32_t*)(p + off); off += align_up(n * 4);
-  size_t sort_bytes = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, sort_bytes, (const KeyT*)nullptr, (KeyT*)nullptr, (const int32_t*)nullptr,
-                                  (int32_t*)nullptr, (int64_t)n, 0, sort_end_bit<KeyT>(tile_bits));
-  w.cub_bytes = sort_bytes;
-  w.cub_temp = (void*)(p + off); off += align_up(sort_bytes);
-  w.total = off;
-  return w;
-}
 
 inline int tile_bits_for(int n_tiles) {  // bits needed to represent the values 0..n_tiles (n_tiles = the padding key)
   int b = 1;
@@ -279,9 +262,10 @@ __global__ void __launch_bounds__(256) offsets_kernel(const KeyT* __restrict__ k
 template <typename KeyT>
 int bin_sort_impl(const DnrArgs* a, cudaStream_t s, int n_tiles, int tile_bits) {
   const int tiles_x = dnr_stiles_x(a), tiles_y = dnr_stiles_y(a);
-  ScanWs sw = carve_scan(a->ws_scan, a->n_gauss);
+  const ScanWs sw(a->ws_scan, a->n_gauss);
   const int64_t cap = a->n_isects;
-  SortWs<KeyT> w = carve_sort<KeyT>(a->ws_sort, cap, tile_bits);
+  const SortWs<KeyT> w(a->ws_sort, cap, tile_bits);
+  if (const int e = w.carve.cub_error()) return e;
   if (cap > 0) {
     emit_kernel<KeyT><<<(unsigned)((a->n_gauss + 255) / 256), 256, 0, s>>>(*a, sw.order, sw.isect_start, w.keys_in, w.gids_in,
                                                                           tiles_x, tiles_y);
@@ -303,7 +287,7 @@ int bin_sort_impl(const DnrArgs* a, cudaStream_t s, int n_tiles, int tile_bits) 
 
 extern "C" size_t dnr_bin_scan_workspace_bytes(int32_t n_gauss) {
   if (n_gauss <= 0) return 0;
-  return carve_scan(nullptr, n_gauss).total;
+  return ScanWs(nullptr, n_gauss).carve.total();
 }
 
 extern "C" int dnr_bin_scan(const DnrArgs* a, void* stream, int64_t* n_isects_host) {
@@ -315,7 +299,8 @@ extern "C" int dnr_bin_scan(const DnrArgs* a, void* stream, int64_t* n_isects_ho
   if (!(a->flags & DNR_FLAG_EXACT_LISTS) && (!a->conics || !a->cull_lim)) return DNR_E_NULL;
   cudaStream_t s = (cudaStream_t)stream;
   const int32_t n = a->n_gauss;
-  ScanWs w = carve_scan(a->ws_scan, n);
+  const ScanWs w(a->ws_scan, n);
+  if (const int e = w.carve.cub_error()) return e;
   iota_kernel<<<(n + 255) / 256, 256, 0, s>>>(w.iota, n);
   DNR_CHECK_LAUNCH();
   size_t bytes = w.cub_bytes;
@@ -344,8 +329,8 @@ extern "C" size_t dnr_bin_sort_workspace_bytes(int32_t n_gauss, int64_t n_isects
   (void)n_gauss;
   if (n_isects < 0 || n_tiles <= 0) return 0;
   const int bits = tile_bits_for(n_tiles);
-  if (n_tiles < 65536) return carve_sort<uint16_t>(nullptr, n_isects, bits).total;
-  return carve_sort<uint32_t>(nullptr, n_isects, bits).total;
+  if (n_tiles < 65536) return SortWs<uint16_t>(nullptr, n_isects, bits).carve.total();
+  return SortWs<uint32_t>(nullptr, n_isects, bits).carve.total();
 }
 
 extern "C" int dnr_bin_sort(const DnrArgs* a, void* stream) {

@@ -24,6 +24,33 @@
     if (e__ != cudaSuccess) return (int)e__;       \
   } while (0)
 
+// Carves a caller-owned workspace into regions, each at the next 256-byte boundary, in the order they are taken.  On a
+// null base it only sizes the workspace.  cub's scratch is taken with the status of its size query: when a query fails
+// the workspace has no room for cub, so check() makes the entry point refuse to run rather than launch cub without it.
+class DnrCarver {
+ public:
+  explicit DnrCarver(const void* base) : base_((uintptr_t)base) {}
+  template <class T>
+  T* take(size_t count) {
+    T* p = base_ ? (T*)(base_ + off_) : nullptr;
+    off_ += (sizeof(T) * count + 255) & ~(size_t)255;
+    return p;
+  }
+  void* cub_scratch(cudaError_t query, size_t bytes) {
+    if (err_ == cudaSuccess) err_ = query;
+    return take<char>(bytes);
+  }
+  size_t total() const { return off_; }
+  int cub_error() const { return (int)err_; }
+  // DNR_E_WORKSPACE when ws_bytes is short of total(), else the first failed cub size query, else 0
+  int check(int64_t ws_bytes) const { return (int64_t)off_ > ws_bytes ? DNR_E_WORKSPACE : cub_error(); }
+
+ private:
+  uintptr_t base_;
+  size_t off_ = 0;
+  cudaError_t err_ = cudaSuccess;
+};
+
 static inline int dnr_tiles_x(const DnrArgs* a) { return (a->width + DNR_TILE - 1) / DNR_TILE; }
 static inline int dnr_tiles_y(const DnrArgs* a) { return (a->height + DNR_TILE - 1) / DNR_TILE; }
 // supertiles: the intersection lists are kept per (16 << list_shift)^2-pixel block

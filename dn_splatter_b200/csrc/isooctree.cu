@@ -33,7 +33,6 @@ constexpr double BACK_MASK_COEFF = 0.25;
 constexpr int LEVEL_SHIFT = 58;
 constexpr int64_t CODE_MASK = (int64_t(1) << LEVEL_SHIFT) - 1;
 
-__host__ size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
 
 struct Pose {  // one row of DnrIsoFrames::poses
   const double* p;
@@ -281,38 +280,38 @@ __global__ void iso_children_kernel(DnrIsoGrid g, int level, const int64_t* __re
 }
 
 struct OctLayout {
+  DnrCarver carve;
   int64_t bound;  // split nodes of one level, at most
-  size_t keys, sorted, lists, children, split, leaf, leaves, num, cub_temp, cub_bytes, total;
-};
-
-OctLayout oct_layout(const DnrIsoGrid* g, int64_t n) {
-  OctLayout L;
-  const int64_t by_count = n / g->threshold;
-  int64_t bound = 1, pw = 1;
-  for (int l = 1; l < g->max_depth; ++l) {
-    pw = pw < (int64_t(1) << 40) ? pw * 8 : pw;
-    bound = std::max(bound, std::min(pw, by_count));
+  int64_t *leaves, *keys, *sorted, *lists, *children, *num;
+  uint8_t *split, *leaf;
+  void* cub_temp;
+  size_t cub_bytes;
+  OctLayout(const void* base, const DnrIsoGrid* g, int64_t n) : carve(base) {
+    const int64_t by_count = n / g->threshold;
+    int64_t b = 1, pw = 1;
+    for (int l = 1; l < g->max_depth; ++l) {
+      pw = pw < (int64_t(1) << 40) ? pw * 8 : pw;
+      b = std::max(b, std::min(pw, by_count));
+    }
+    bound = std::max<int64_t>(b, 1);
+    // first, so that their place does not depend on n: dnr_iso_corners reads them from the octree's workspace
+    leaves = carve.take<int64_t>((int64_t)g->max_depth * 8 * bound + 1);  // leaves of all levels
+    keys = carve.take<int64_t>(std::max<int64_t>(n, 1));
+    sorted = carve.take<int64_t>(std::max<int64_t>(n, 1));
+    lists = carve.take<int64_t>(2 * bound);  // this level's split nodes and the next's
+    children = carve.take<int64_t>(8 * bound);
+    split = carve.take<uint8_t>(8 * bound);
+    leaf = carve.take<uint8_t>(8 * bound);
+    num = carve.take<int64_t>(2);
+    size_t t_sort = 0, t_sel = 0;
+    const cudaError_t e1 = cub::DeviceRadixSort::SortKeys(nullptr, t_sort, (const int64_t*)nullptr, (int64_t*)nullptr,
+                                                          (int64_t)std::max<int64_t>(n, 1));
+    const cudaError_t e2 = cub::DeviceSelect::Flagged(nullptr, t_sel, (const int64_t*)nullptr, (const uint8_t*)nullptr,
+                                                      (int64_t*)nullptr, (int64_t*)nullptr, (int64_t)(8 * bound));
+    cub_bytes = std::max(t_sort, t_sel);
+    cub_temp = carve.cub_scratch(e1 != cudaSuccess ? e1 : e2, cub_bytes);
   }
-  L.bound = std::max<int64_t>(bound, 1);
-  const int64_t nl = (int64_t)g->max_depth * 8 * L.bound + 1;  // leaves of all levels
-  size_t o = 0;
-  L.leaves = o; o = align256(o + 8 * (size_t)nl);  // first: dnr_iso_corners reads the leaves at the workspace's start
-  L.keys = o; o = align256(o + 8 * (size_t)std::max<int64_t>(n, 1));
-  L.sorted = o; o = align256(o + 8 * (size_t)std::max<int64_t>(n, 1));
-  L.lists = o; o = align256(o + 2 * 8 * (size_t)L.bound);  // this level's split nodes and the next's
-  L.children = o; o = align256(o + 8 * 8 * (size_t)L.bound);
-  L.split = o; o = align256(o + 8 * (size_t)L.bound);
-  L.leaf = o; o = align256(o + 8 * (size_t)L.bound);
-  L.num = o; o = align256(o + 2 * sizeof(int64_t));
-  size_t t_sort = 0, t_sel = 0;
-  cub::DeviceRadixSort::SortKeys(nullptr, t_sort, (const int64_t*)nullptr, (int64_t*)nullptr, (int64_t)std::max<int64_t>(n, 1));
-  cub::DeviceSelect::Flagged(nullptr, t_sel, (const int64_t*)nullptr, (const uint8_t*)nullptr, (int64_t*)nullptr,
-                             (int64_t*)nullptr, (int64_t)(8 * L.bound));
-  L.cub_bytes = std::max(t_sort, t_sel);
-  L.cub_temp = o; o = align256(o + L.cub_bytes);
-  L.total = o;
-  return L;
-}
+};
 
 int check_grid(const DnrIsoGrid* g) {
   if (!g) return DNR_E_NULL;
@@ -331,45 +330,42 @@ constexpr int THREADS = 256;
 unsigned blocks_for(int64_t n, int t = THREADS) { return (unsigned)((n + t - 1) / t); }
 
 struct SampleLayout {
-  size_t flags, idx, num, cub_temp, cub_bytes, total;
+  DnrCarver carve;
+  uint8_t* flags;
+  int64_t *idx, *num;
+  void* cub_temp;
+  size_t cub_bytes = 0;
+  SampleLayout(void* base, int64_t total) : carve(base) {
+    flags = carve.take<uint8_t>(total);
+    idx = carve.take<int64_t>(total);
+    num = carve.take<int64_t>(1);
+    const cudaError_t e = cub::DeviceSelect::Flagged(nullptr, cub_bytes, thrust::counting_iterator<int64_t>(0), (const uint8_t*)nullptr,
+                                                     (int64_t*)nullptr, (int64_t*)nullptr, total);
+    cub_temp = carve.cub_scratch(e, cub_bytes);
+  }
 };
-
-SampleLayout sample_layout(int64_t total) {
-  SampleLayout L;
-  size_t o = 0, t = 0;
-  L.flags = o; o = align256(o + (size_t)total);
-  L.idx = o; o = align256(o + 8 * (size_t)total);
-  L.num = o; o = align256(o + 8);
-  cub::DeviceSelect::Flagged(nullptr, t, thrust::counting_iterator<int64_t>(0), (const uint8_t*)nullptr, (int64_t*)nullptr,
-                             (int64_t*)nullptr, total);
-  L.cub_bytes = t;
-  L.cub_temp = o; o = align256(o + t);
-  L.total = o;
-  return L;
-}
 
 int64_t sample_total(const DnrIsoFrames* fr, int stride) {
   return (int64_t)fr->n_frames * ((fr->height + stride - 1) / stride) * ((fr->width + stride - 1) / stride);
 }
 
 struct CornerLayout {
-  size_t keys8, sorted, num, cub_temp, cub_bytes, total;
+  DnrCarver carve;
+  int64_t *keys8, *sorted, *num;
+  void* cub_temp;
+  size_t cub_bytes;
+  CornerLayout(void* base, int64_t n_leaves) : carve(base) {
+    const int64_t m = std::max<int64_t>(8 * n_leaves, 1);
+    keys8 = carve.take<int64_t>(m);
+    sorted = carve.take<int64_t>(m);
+    num = carve.take<int64_t>(1);
+    size_t t_sort = 0, t_uni = 0;
+    const cudaError_t e1 = cub::DeviceRadixSort::SortKeys(nullptr, t_sort, (const int64_t*)nullptr, (int64_t*)nullptr, m);
+    const cudaError_t e2 = cub::DeviceSelect::Unique(nullptr, t_uni, (const int64_t*)nullptr, (int64_t*)nullptr, (int64_t*)nullptr, m);
+    cub_bytes = std::max(t_sort, t_uni);
+    cub_temp = carve.cub_scratch(e1 != cudaSuccess ? e1 : e2, cub_bytes);
+  }
 };
-
-CornerLayout corner_layout(int64_t n_leaves) {
-  CornerLayout L;
-  const int64_t m = std::max<int64_t>(8 * n_leaves, 1);
-  size_t o = 0, t_sort = 0, t_uni = 0;
-  L.keys8 = o; o = align256(o + 8 * (size_t)m);
-  L.sorted = o; o = align256(o + 8 * (size_t)m);
-  L.num = o; o = align256(o + 8);
-  cub::DeviceRadixSort::SortKeys(nullptr, t_sort, (const int64_t*)nullptr, (int64_t*)nullptr, m);
-  cub::DeviceSelect::Unique(nullptr, t_uni, (const int64_t*)nullptr, (int64_t*)nullptr, (int64_t*)nullptr, m);
-  L.cub_bytes = std::max(t_sort, t_uni);
-  L.cub_temp = o; o = align256(o + L.cub_bytes);
-  L.total = o;
-  return L;
-}
 
 __device__ __forceinline__ void leaf_box(int64_t leaf, int D, int64_t* lo, int64_t* size) {
   const int level = (int)(leaf >> LEVEL_SHIFT);
@@ -434,7 +430,7 @@ extern "C" int64_t dnr_iso_samples_workspace_bytes(const DnrIsoFrames* fr, int32
   const int rc = check_frames(fr);
   if (rc) return rc;
   if (stride <= 0) return DNR_E_SIZE;
-  return (int64_t)sample_layout(sample_total(fr, stride)).total;
+  return (int64_t)SampleLayout(nullptr, sample_total(fr, stride)).carve.total();
 }
 
 extern "C" int dnr_iso_samples(const DnrIsoFrames* fr, int32_t stride, void* ws, int64_t ws_bytes, double* points, double* normals,
@@ -444,18 +440,16 @@ extern "C" int dnr_iso_samples(const DnrIsoFrames* fr, int32_t stride, void* ws,
   if (stride <= 0) return DNR_E_SIZE;
   if (!ws || !points || !count_host) return DNR_E_NULL;
   const int64_t total = sample_total(fr, stride);
-  const SampleLayout L = sample_layout(total);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
+  const SampleLayout L(ws, total);
+  if (const int e = L.carve.check(ws_bytes)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  char* w = (char*)ws;
-  uint8_t* flags = (uint8_t*)(w + L.flags);
-  int64_t* idx = (int64_t*)(w + L.idx);
-  int64_t* num = (int64_t*)(w + L.num);
+  uint8_t* flags = L.flags;
+  int64_t *idx = L.idx, *num = L.num;
   const int ws_ = (fr->width + stride - 1) / stride, hs = (fr->height + stride - 1) / stride;
   iso_sample_flags_kernel<<<blocks_for(total), THREADS, 0, s>>>(*fr, stride, ws_, hs, total, flags);
   DNR_CHECK_LAUNCH();
   size_t t = L.cub_bytes;
-  DNR_CUDA(cub::DeviceSelect::Flagged(w + L.cub_temp, t, thrust::counting_iterator<int64_t>(0), flags, idx, num, total, s));
+  DNR_CUDA(cub::DeviceSelect::Flagged(L.cub_temp, t, thrust::counting_iterator<int64_t>(0), flags, idx, num, total, s));
   DNR_CUDA(cudaMemcpyAsync(count_host, num, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
   DNR_CUDA(cudaStreamSynchronize(s));
   if (*count_host > 0) {
@@ -483,7 +477,7 @@ extern "C" int64_t dnr_iso_octree_workspace_bytes(const DnrIsoGrid* g, int64_t n
   const int rc = check_grid(g);
   if (rc) return rc;
   if (n < 0) return DNR_E_SIZE;
-  return (int64_t)oct_layout(g, n).total;
+  return (int64_t)OctLayout(nullptr, g, n).carve.total();
 }
 
 extern "C" int dnr_iso_octree(const DnrIsoGrid* g, const double* points, int64_t n, void* ws, int64_t ws_bytes,
@@ -492,18 +486,12 @@ extern "C" int dnr_iso_octree(const DnrIsoGrid* g, const double* points, int64_t
   if (rc) return rc;
   if (n < 0) return DNR_E_SIZE;
   if (!ws || !level_counts_host || (n > 0 && !points)) return DNR_E_NULL;
-  const OctLayout L = oct_layout(g, n);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
+  const OctLayout L(ws, g, n);
+  if (const int e = L.carve.check(ws_bytes)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  char* w = (char*)ws;
-  int64_t* keys = (int64_t*)(w + L.keys);
-  int64_t* sorted = (int64_t*)(w + L.sorted);
-  int64_t* lists[2] = {(int64_t*)(w + L.lists), (int64_t*)(w + L.lists) + L.bound};
-  int64_t* children = (int64_t*)(w + L.children);
-  uint8_t* split = (uint8_t*)(w + L.split);
-  uint8_t* leaf = (uint8_t*)(w + L.leaf);
-  int64_t* leaves = (int64_t*)(w + L.leaves);
-  int64_t* num = (int64_t*)(w + L.num);
+  int64_t *keys = L.keys, *sorted = L.sorted, *children = L.children, *leaves = L.leaves, *num = L.num;
+  int64_t* lists[2] = {L.lists, L.lists + L.bound};
+  uint8_t *split = L.split, *leaf = L.leaf;
   const int D = g->max_depth;
   for (int l = 0; l <= D; ++l) level_counts_host[l] = 0;
   if (!(n >= g->threshold && D > 0)) {  // the root is the only leaf
@@ -514,7 +502,7 @@ extern "C" int dnr_iso_octree(const DnrIsoGrid* g, const double* points, int64_t
   iso_keys_kernel<<<blocks_for(n), THREADS, 0, s>>>(*g, points, n, keys);
   DNR_CHECK_LAUNCH();
   size_t t = L.cub_bytes;
-  DNR_CUDA(cub::DeviceRadixSort::SortKeys(w + L.cub_temp, t, keys, sorted, n, 0, 3 * D, s));
+  DNR_CUDA(cub::DeviceRadixSort::SortKeys(L.cub_temp, t, keys, sorted, n, 0, 3 * D, s));
   DNR_CUDA(cudaMemsetAsync(lists[0], 0, sizeof(int64_t), s));  // the root, level 0, code 0
   int64_t n_parents = 1, n_leaves = 0;
   for (int l = 1; l <= D; ++l) {
@@ -522,9 +510,9 @@ extern "C" int dnr_iso_octree(const DnrIsoGrid* g, const double* points, int64_t
     iso_children_kernel<<<blocks_for(m), THREADS, 0, s>>>(*g, l, lists[(l - 1) & 1], n_parents, sorted, n, children, split, leaf);
     DNR_CHECK_LAUNCH();
     t = L.cub_bytes;
-    DNR_CUDA(cub::DeviceSelect::Flagged(w + L.cub_temp, t, children, split, lists[l & 1], num, m, s));
+    DNR_CUDA(cub::DeviceSelect::Flagged(L.cub_temp, t, children, split, lists[l & 1], num, m, s));
     t = L.cub_bytes;
-    DNR_CUDA(cub::DeviceSelect::Flagged(w + L.cub_temp, t, children, leaf, leaves + n_leaves, num + 1, m, s));
+    DNR_CUDA(cub::DeviceSelect::Flagged(L.cub_temp, t, children, leaf, leaves + n_leaves, num + 1, m, s));
     int64_t got[2];
     DNR_CUDA(cudaMemcpyAsync(got, num, sizeof(got), cudaMemcpyDeviceToHost, s));
     DNR_CUDA(cudaStreamSynchronize(s));
@@ -541,7 +529,7 @@ extern "C" int64_t dnr_iso_corners_workspace_bytes(const DnrIsoGrid* g, int64_t 
   const int rc = check_grid(g);
   if (rc) return rc;
   if (n_leaves <= 0) return DNR_E_SIZE;
-  return (int64_t)corner_layout(n_leaves).total;
+  return (int64_t)CornerLayout(nullptr, n_leaves).carve.total();
 }
 
 extern "C" int dnr_iso_corners(const DnrIsoGrid* g, const void* octree_ws, const int64_t* level_counts_host, void* ws,
@@ -554,15 +542,13 @@ extern "C" int dnr_iso_corners(const DnrIsoGrid* g, const void* octree_ws, const
   int64_t n_leaves = 0;
   for (int l = 0; l <= g->max_depth; ++l) n_leaves += level_counts_host[l];
   if (n_leaves <= 0) return DNR_E_SIZE;
-  const CornerLayout L = corner_layout(n_leaves);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
+  const CornerLayout L(ws, n_leaves);
+  if (const int e = L.carve.check(ws_bytes)) return e;
   if (8 * n_leaves > INT32_MAX) return DNR_E_OVERFLOW;
   cudaStream_t s = (cudaStream_t)stream;
-  char* w = (char*)ws;
-  int64_t* keys8 = (int64_t*)(w + L.keys8);
-  int64_t* sorted = (int64_t*)(w + L.sorted);
-  int64_t* num = (int64_t*)(w + L.num);
-  DNR_CUDA(cudaMemcpyAsync(leaves, octree_ws, sizeof(int64_t) * n_leaves, cudaMemcpyDeviceToDevice, s));
+  int64_t *keys8 = L.keys8, *sorted = L.sorted, *num = L.num;
+  const int64_t* octree_leaves = OctLayout(octree_ws, g, 0).leaves;
+  DNR_CUDA(cudaMemcpyAsync(leaves, octree_leaves, sizeof(int64_t) * n_leaves, cudaMemcpyDeviceToDevice, s));
   const int D = g->max_depth;
   const int64_t m = 8 * n_leaves;
   iso_corner_keys_kernel<<<blocks_for(m), THREADS, 0, s>>>(D, leaves, n_leaves, keys8);
@@ -570,9 +556,9 @@ extern "C" int dnr_iso_corners(const DnrIsoGrid* g, const void* octree_ws, const
   int bits = 1;
   while (bits < 63 && (int64_t(1) << bits) < ((int64_t(1) << D) + 1) * ((int64_t(1) << D) + 1) * ((int64_t(1) << D) + 1)) ++bits;
   size_t t = L.cub_bytes;
-  DNR_CUDA(cub::DeviceRadixSort::SortKeys(w + L.cub_temp, t, keys8, sorted, m, 0, bits, s));
+  DNR_CUDA(cub::DeviceRadixSort::SortKeys(L.cub_temp, t, keys8, sorted, m, 0, bits, s));
   t = L.cub_bytes;
-  DNR_CUDA(cub::DeviceSelect::Unique(w + L.cub_temp, t, sorted, corner_keys, num, m, s));
+  DNR_CUDA(cub::DeviceSelect::Unique(L.cub_temp, t, sorted, corner_keys, num, m, s));
   iso_corner_index_kernel<<<blocks_for(m), THREADS, 0, s>>>(keys8, m, corner_keys, num, leaf_corners);
   DNR_CHECK_LAUNCH();
   iso_corner_points_kernel<<<blocks_for(m), THREADS, 0, s>>>(*g, corner_keys, num, corner_points);

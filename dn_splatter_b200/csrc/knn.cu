@@ -29,31 +29,27 @@ namespace {
 
 constexpr int KNN_MAX = 33;  // k <= 32 plus the dropped self / nearest column
 
+// dnr_knn_query reads the grid (pts_sorted, cell_start, cell_end) that dnr_knn_build left in the same workspace
 struct KnnLayout {
-  size_t cell_ids, cell_ids_sorted, order, order_sorted, pts_sorted, cell_start, cell_end, cub_temp, total;
-  size_t cub_bytes;
+  DnrCarver carve;
+  uint32_t *cell_ids, *cell_ids_sorted;
+  int32_t *order, *order_sorted, *cell_start, *cell_end;
+  float4* pts_sorted;
+  void* cub_temp;
+  size_t cub_bytes = 0;
+  KnnLayout(const void* base, int32_t n, int64_t n_cells) : carve(base) {
+    cell_ids = carve.take<uint32_t>(n);
+    cell_ids_sorted = carve.take<uint32_t>(n);
+    order = carve.take<int32_t>(n);
+    order_sorted = carve.take<int32_t>(n);
+    pts_sorted = carve.take<float4>(n);
+    cell_start = carve.take<int32_t>(n_cells);
+    cell_end = carve.take<int32_t>(n_cells);
+    const cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                                          (const int32_t*)nullptr, (int32_t*)nullptr, n, 0, 32);
+    cub_temp = carve.cub_scratch(e, cub_bytes);
+  }
 };
-
-__host__ size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
-KnnLayout knn_layout(int32_t n, int64_t n_cells) {
-  KnnLayout L;
-  size_t off = 0;
-  L.cell_ids = off; off = align256(off + sizeof(uint32_t) * (size_t)n);
-  L.cell_ids_sorted = off; off = align256(off + sizeof(uint32_t) * (size_t)n);
-  L.order = off; off = align256(off + sizeof(int32_t) * (size_t)n);
-  L.order_sorted = off; off = align256(off + sizeof(int32_t) * (size_t)n);
-  L.pts_sorted = off; off = align256(off + sizeof(float4) * (size_t)n);
-  L.cell_start = off; off = align256(off + sizeof(int32_t) * (size_t)n_cells);
-  L.cell_end = off; off = align256(off + sizeof(int32_t) * (size_t)n_cells);
-  size_t temp = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, temp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
-                                  (int32_t*)nullptr, n, 0, 32);
-  L.cub_bytes = temp;
-  L.cub_temp = off; off = align256(off + temp);
-  L.total = off;
-  return L;
-}
 
 __device__ __forceinline__ int cell_coord(float x, float lo, float inv_cell, int dim) {
   const int c = (int)floorf((x - lo) * inv_cell);
@@ -167,7 +163,7 @@ int check_grid(const DnrKnnGrid* g, int64_t* n_cells) {
 extern "C" int64_t dnr_knn_workspace_bytes(int32_t n_points, const DnrKnnGrid* grid) {
   int64_t n_cells = 0;
   if (n_points <= 0 || check_grid(grid, &n_cells)) return -1;
-  return (int64_t)knn_layout(n_points, n_cells).total;
+  return (int64_t)KnnLayout(nullptr, n_points, n_cells).carve.total();
 }
 
 extern "C" int dnr_knn_build(const float* points, int32_t n_points, const DnrKnnGrid* grid, void* ws, int64_t ws_bytes, void* stream) {
@@ -176,25 +172,21 @@ extern "C" int dnr_knn_build(const float* points, int32_t n_points, const DnrKnn
   int64_t n_cells = 0;
   const int rc = check_grid(grid, &n_cells);
   if (rc) return rc;
-  const KnnLayout L = knn_layout(n_points, n_cells);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
+  const KnnLayout L(ws, n_points, n_cells);
+  if (const int e = L.carve.check(ws_bytes)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  char* base = (char*)ws;
-  uint32_t* cell_ids = (uint32_t*)(base + L.cell_ids);
-  uint32_t* cell_sorted = (uint32_t*)(base + L.cell_ids_sorted);
-  int32_t* order = (int32_t*)(base + L.order);
-  int32_t* order_sorted = (int32_t*)(base + L.order_sorted);
   const int blocks = (n_points + 255) / 256;
-  knn_bin_kernel<<<blocks, 256, 0, s>>>(points, n_points, *grid, cell_ids, order);
+  knn_bin_kernel<<<blocks, 256, 0, s>>>(points, n_points, *grid, L.cell_ids, L.order);
   DNR_CHECK_LAUNCH();
   size_t temp = L.cub_bytes;
   int bits = 1;
   while (((int64_t)1 << bits) < n_cells) ++bits;
-  DNR_CUDA(cub::DeviceRadixSort::SortPairs(base + L.cub_temp, temp, cell_ids, cell_sorted, order, order_sorted, n_points, 0, bits, s));
-  DNR_CUDA(cudaMemsetAsync(base + L.cell_start, 0, sizeof(int32_t) * (size_t)n_cells, s));
-  DNR_CUDA(cudaMemsetAsync(base + L.cell_end, 0, sizeof(int32_t) * (size_t)n_cells, s));
-  knn_ranges_kernel<<<blocks, 256, 0, s>>>(points, n_points, cell_sorted, order_sorted, (float4*)(base + L.pts_sorted),
-                                           (int32_t*)(base + L.cell_start), (int32_t*)(base + L.cell_end));
+  DNR_CUDA(cub::DeviceRadixSort::SortPairs(L.cub_temp, temp, L.cell_ids, L.cell_ids_sorted, L.order, L.order_sorted, n_points, 0,
+                                           bits, s));
+  DNR_CUDA(cudaMemsetAsync(L.cell_start, 0, sizeof(int32_t) * (size_t)n_cells, s));
+  DNR_CUDA(cudaMemsetAsync(L.cell_end, 0, sizeof(int32_t) * (size_t)n_cells, s));
+  knn_ranges_kernel<<<blocks, 256, 0, s>>>(points, n_points, L.cell_ids_sorted, L.order_sorted, L.pts_sorted, L.cell_start,
+                                           L.cell_end);
   DNR_CHECK_LAUNCH();
   return 0;
 }
@@ -208,11 +200,9 @@ extern "C" int dnr_knn_query(int32_t n_points, const DnrKnnGrid* grid, const voi
   int64_t n_cells = 0;
   const int rc = check_grid(grid, &n_cells);
   if (rc) return rc;
-  const KnnLayout L = knn_layout(n_points, n_cells);
-  const char* base = (const char*)ws;
-  knn_query_kernel<<<(n_queries + 127) / 128, 128, 0, (cudaStream_t)stream>>>(
-      queries, n_queries, *grid, K, skip_first ? 1 : 0, (const float4*)(base + L.pts_sorted), (const int32_t*)(base + L.cell_start),
-      (const int32_t*)(base + L.cell_end), out_idx, out_dist);
+  const KnnLayout L(ws, n_points, n_cells);
+  knn_query_kernel<<<(n_queries + 127) / 128, 128, 0, (cudaStream_t)stream>>>(queries, n_queries, *grid, K, skip_first ? 1 : 0,
+                                                                              L.pts_sorted, L.cell_start, L.cell_end, out_idx, out_dist);
   DNR_CHECK_LAUNCH();
   return 0;
 }

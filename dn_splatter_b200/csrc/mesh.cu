@@ -279,8 +279,6 @@ __global__ void __launch_bounds__(MC_THREADS) mc_faces_kernel(F f, Geo g, const 
   }
 }
 
-__host__ size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
 int check_field(const DnrMcField* f, Geo* g) {
   if (!f) return DNR_E_NULL;
   if ((f->values == nullptr) == (f->tsdf == nullptr)) return DNR_E_NULL;  // exactly one of them
@@ -296,48 +294,39 @@ int check_field(const DnrMcField* f, Geo* g) {
   return 0;
 }
 
+// dnr_mc_emit reads the exclusive scans `off` that dnr_mc_count left in its workspace
 struct CountLayout {
-  size_t cnt, off, cub_temp, cub_bytes, total;
+  DnrCarver carve;
+  int64_t *cnt, *off;
+  void* cub_temp;
+  size_t cub_bytes = 0;
+  CountLayout(const void* base, int64_t R) : carve(base) {
+    cnt = carve.take<int64_t>(3 * (size_t)(R + 1));
+    off = carve.take<int64_t>(3 * (size_t)(R + 1));
+    const cudaError_t e = cub::DeviceScan::ExclusiveSum(nullptr, cub_bytes, (const int64_t*)nullptr, (int64_t*)nullptr, (int64_t)(R + 1));
+    cub_temp = carve.cub_scratch(e, cub_bytes);
+  }
 };
-
-CountLayout count_layout(int64_t R) {
-  CountLayout L;
-  const size_t n = 3 * (size_t)(R + 1);
-  size_t o = 0;
-  L.cnt = o; o = align256(o + sizeof(int64_t) * n);
-  L.off = o; o = align256(o + sizeof(int64_t) * n);
-  size_t temp = 0;
-  cub::DeviceScan::ExclusiveSum(nullptr, temp, (const int64_t*)nullptr, (int64_t*)nullptr, (int64_t)(R + 1));
-  L.cub_bytes = temp;
-  L.cub_temp = o; o = align256(o + temp);
-  L.total = o;
-  return L;
-}
 
 struct EmitLayout {
-  size_t cube_ids, tri_start, vkeys, total;
+  DnrCarver carve;
+  int64_t *cube_ids, *tri_start, *vkeys;
+  EmitLayout(void* base, int64_t n_cubes, int64_t n_verts) : carve(base) {
+    cube_ids = carve.take<int64_t>(n_cubes);
+    tri_start = carve.take<int64_t>(n_cubes);
+    vkeys = carve.take<int64_t>(n_verts);
+  }
 };
 
-EmitLayout emit_layout(int64_t n_cubes, int64_t n_verts) {
-  EmitLayout L;
-  size_t o = 0;
-  L.cube_ids = o; o = align256(o + sizeof(int64_t) * (size_t)n_cubes);
-  L.tri_start = o; o = align256(o + sizeof(int64_t) * (size_t)n_cubes);
-  L.vkeys = o; o = align256(o + sizeof(int64_t) * (size_t)n_verts);
-  L.total = o;
-  return L;
-}
-
 template <class F>
-int mc_count(const F& f, const Geo& g, char* ws, const CountLayout& L, int64_t* counts_host, cudaStream_t s) {
+int mc_count(const F& f, const Geo& g, const CountLayout& L, int64_t* counts_host, cudaStream_t s) {
   const int64_t R = (int64_t)g.X * g.Y;
-  int64_t* cnt = (int64_t*)(ws + L.cnt);
-  int64_t* off = (int64_t*)(ws + L.off);
+  int64_t *cnt = L.cnt, *off = L.off;
   mc_count_kernel<F><<<dim3(g.Y, g.X), MC_THREADS, 0, s>>>(f, g, cnt, R);
   DNR_CHECK_LAUNCH();
   for (int a = 0; a < 3; ++a) {
     size_t temp = L.cub_bytes;
-    DNR_CUDA(cub::DeviceScan::ExclusiveSum(ws + L.cub_temp, temp, cnt + a * (R + 1), off + a * (R + 1), (int64_t)(R + 1), s));
+    DNR_CUDA(cub::DeviceScan::ExclusiveSum(L.cub_temp, temp, cnt + a * (R + 1), off + a * (R + 1), (int64_t)(R + 1), s));
   }
   for (int a = 0; a < 3; ++a)
     DNR_CUDA(cudaMemcpyAsync(counts_host + a, off + a * (R + 1) + R, sizeof(int64_t), cudaMemcpyDeviceToHost, s));
@@ -346,17 +335,14 @@ int mc_count(const F& f, const Geo& g, char* ws, const CountLayout& L, int64_t* 
 }
 
 template <class F>
-int mc_emit(const F& f, const Geo& g, const int64_t* off, const int64_t* counts, char* ws, const EmitLayout& L, float* verts,
-            int32_t* faces, float* colors, cudaStream_t s) {
+int mc_emit(const F& f, const Geo& g, const int64_t* off, const int64_t* counts, const EmitLayout& L, float* verts, int32_t* faces,
+            float* colors, cudaStream_t s) {
   const int64_t R = (int64_t)g.X * g.Y;
-  int64_t* cube_ids = (int64_t*)(ws + L.cube_ids);
-  int64_t* tri_start = (int64_t*)(ws + L.tri_start);
-  int64_t* vkeys = (int64_t*)(ws + L.vkeys);
-  mc_compact_kernel<F><<<dim3(g.Y, g.X), MC_THREADS, 0, s>>>(f, g, off, R, cube_ids, tri_start, vkeys, verts, colors);
+  mc_compact_kernel<F><<<dim3(g.Y, g.X), MC_THREADS, 0, s>>>(f, g, off, R, L.cube_ids, L.tri_start, L.vkeys, verts, colors);
   DNR_CHECK_LAUNCH();
   if (counts[0] > 0) {
-    mc_faces_kernel<F><<<(unsigned)((counts[0] + 127) / 128), 128, 0, s>>>(f, g, cube_ids, tri_start, counts[0],
-                                                                          off + 2 * (R + 1), vkeys, faces);
+    mc_faces_kernel<F><<<(unsigned)((counts[0] + 127) / 128), 128, 0, s>>>(f, g, L.cube_ids, L.tri_start, counts[0],
+                                                                          off + 2 * (R + 1), L.vkeys, faces);
     DNR_CHECK_LAUNCH();
   }
   return 0;
@@ -386,7 +372,7 @@ extern "C" int64_t dnr_mc_count_workspace_bytes(const DnrMcField* field) {
   Geo g;
   const int rc = check_field(field, &g);
   if (rc) return rc;
-  return (int64_t)count_layout((int64_t)g.X * g.Y).total;
+  return (int64_t)CountLayout(nullptr, (int64_t)g.X * g.Y).carve.total();
 }
 
 extern "C" int dnr_mc_count(const DnrMcField* field, void* ws, int64_t ws_bytes, int64_t* counts_host, void* stream) {
@@ -394,17 +380,17 @@ extern "C" int dnr_mc_count(const DnrMcField* field, void* ws, int64_t ws_bytes,
   const int rc = check_field(field, &g);
   if (rc) return rc;
   if (!ws || !counts_host) return DNR_E_NULL;
-  const CountLayout L = count_layout((int64_t)g.X * g.Y);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
+  const CountLayout L(ws, (int64_t)g.X * g.Y);
+  if (const int e = L.carve.check(ws_bytes)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  if (field->tsdf) return mc_count(TsdfField{(const float4*)field->tsdf}, g, (char*)ws, L, counts_host, s);
-  return mc_count(ScalarField{field->values, field->valid}, g, (char*)ws, L, counts_host, s);
+  if (field->tsdf) return mc_count(TsdfField{(const float4*)field->tsdf}, g, L, counts_host, s);
+  return mc_count(ScalarField{field->values, field->valid}, g, L, counts_host, s);
 }
 
 extern "C" int64_t dnr_mc_emit_workspace_bytes(const int64_t* counts_host) {
   if (!counts_host) return DNR_E_NULL;
   if (counts_host[0] < 0 || counts_host[1] < 0 || counts_host[2] < 0) return DNR_E_SIZE;
-  return (int64_t)emit_layout(counts_host[0], counts_host[2]).total;
+  return (int64_t)EmitLayout(nullptr, counts_host[0], counts_host[2]).carve.total();
 }
 
 extern "C" int dnr_mc_emit(const DnrMcField* field, const void* count_ws, const int64_t* counts_host, void* ws, int64_t ws_bytes,
@@ -416,12 +402,10 @@ extern "C" int dnr_mc_emit(const DnrMcField* field, const void* count_ws, const 
   if (counts_host[0] < 0 || counts_host[1] < 0 || counts_host[2] < 0) return DNR_E_SIZE;
   if (counts_host[1] > INT32_MAX || counts_host[2] > INT32_MAX) return DNR_E_OVERFLOW;
   if ((counts_host[1] > 0 && !faces) || (counts_host[2] > 0 && !vertices)) return DNR_E_NULL;
-  const EmitLayout L = emit_layout(counts_host[0], counts_host[2]);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
-  const CountLayout CL = count_layout((int64_t)g.X * g.Y);
-  const int64_t* off = (const int64_t*)((const char*)count_ws + CL.off);
+  const EmitLayout L(ws, counts_host[0], counts_host[2]);
+  if (const int e = L.carve.check(ws_bytes)) return e;
+  const int64_t* off = CountLayout(count_ws, (int64_t)g.X * g.Y).off;
   cudaStream_t s = (cudaStream_t)stream;
-  if (field->tsdf)
-    return mc_emit(TsdfField{(const float4*)field->tsdf}, g, off, counts_host, (char*)ws, L, vertices, faces, colors, s);
-  return mc_emit(ScalarField{field->values, field->valid}, g, off, counts_host, (char*)ws, L, vertices, faces, nullptr, s);
+  if (field->tsdf) return mc_emit(TsdfField{(const float4*)field->tsdf}, g, off, counts_host, L, vertices, faces, colors, s);
+  return mc_emit(ScalarField{field->values, field->valid}, g, off, counts_host, L, vertices, faces, nullptr, s);
 }

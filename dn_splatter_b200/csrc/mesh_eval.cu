@@ -32,25 +32,22 @@ constexpr int VIS_THREADS = 128;
 
 // Workspace of dnr_mesh_depth.  tests/test_gpu_mesh_eval_kernels.py reads the last view's boxes, counts and scan back
 // from it at these offsets (int4 boxes at 0, then the int64 arrays at 256-B boundaries): change both together.
+// Workspace of dnr_mesh_depth.  tests/test_gpu_mesh_eval_kernels.py reads the last view's boxes, counts and scan back
+// from it at these offsets (int4 boxes at 0, then the int64 arrays at 256-B boundaries): change both together.
 struct DepthLayout {
-  size_t boxes, counts, scan, cub_temp, total, cub_bytes;
+  DnrCarver carve;
+  int4* boxes;
+  int64_t *counts, *scan;
+  void* cub_temp;
+  size_t cub_bytes = 0;
+  DepthLayout(void* base, int64_t n_faces) : carve(base) {
+    boxes = carve.take<int4>(n_faces);
+    counts = carve.take<int64_t>(n_faces);
+    scan = carve.take<int64_t>(n_faces);
+    const cudaError_t e = cub::DeviceScan::InclusiveSum(nullptr, cub_bytes, (const int64_t*)nullptr, (int64_t*)nullptr, n_faces);
+    cub_temp = carve.cub_scratch(e, cub_bytes);
+  }
 };
-
-size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
-DepthLayout depth_layout(int64_t n_faces) {
-  DepthLayout L;
-  size_t off = 0;
-  L.boxes = off; off = align256(off + sizeof(int4) * (size_t)n_faces);
-  L.counts = off; off = align256(off + sizeof(int64_t) * (size_t)n_faces);
-  L.scan = off; off = align256(off + sizeof(int64_t) * (size_t)n_faces);
-  size_t temp = 0;
-  cub::DeviceScan::InclusiveSum(nullptr, temp, (const int64_t*)nullptr, (int64_t*)nullptr, (int64_t)n_faces);
-  L.cub_bytes = temp;
-  L.cub_temp = off; off = align256(off + temp);
-  L.total = off;
-  return L;
-}
 
 __device__ __forceinline__ double3 to_camera(const float* __restrict__ cam, const float* __restrict__ verts, int v) {
   const double x = verts[3 * v], y = verts[3 * v + 1], z = verts[3 * v + 2];
@@ -217,7 +214,7 @@ __global__ void __launch_bounds__(VIS_THREADS) visibility_kernel(const double* _
 
 extern "C" int64_t dnr_mesh_depth_workspace_bytes(int64_t n_faces) {
   if (n_faces <= 0) return DNR_E_SIZE;
-  return (int64_t)depth_layout(n_faces).total;
+  return (int64_t)DepthLayout(nullptr, n_faces).carve.total();
 }
 
 extern "C" int dnr_mesh_depth(const float* vertices, int32_t n_vertices, const int32_t* faces, int64_t n_faces, const float* cams,
@@ -226,13 +223,9 @@ extern "C" int dnr_mesh_depth(const float* vertices, int32_t n_vertices, const i
   if (!vertices || !faces || !cams || !ws || !depth) return DNR_E_NULL;
   if (n_vertices <= 0 || n_faces <= 0 || n_views <= 0 || width <= 0 || height <= 0) return DNR_E_SIZE;
   if (!(near > 0.f) || !(far >= near)) return DNR_E_OPTION;
-  const DepthLayout L = depth_layout(n_faces);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
+  const DepthLayout L(ws, n_faces);
+  if (const int e = L.carve.check(ws_bytes)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  char* base = (char*)ws;
-  int4* boxes = (int4*)(base + L.boxes);
-  int64_t* counts = (int64_t*)(base + L.counts);
-  int64_t* scan = (int64_t*)(base + L.scan);
   const int64_t pixels = (int64_t)width * height;
   uint32_t* zbuf = reinterpret_cast<uint32_t*>(depth);
   DNR_CUDA(cudaMemsetAsync(zbuf, 0xFF, sizeof(uint32_t) * (size_t)(pixels * n_views), s));
@@ -241,12 +234,12 @@ extern "C" int dnr_mesh_depth(const float* vertices, int32_t n_vertices, const i
   for (int v = 0; v < n_views; ++v) {
     const float* cam = cams + 16 * (int64_t)v;
     depth_box_kernel<<<(unsigned)box_blocks, BOX_THREADS, 0, s>>>(vertices, n_vertices, faces, n_faces, cam, width, height, near, far,
-                                                                  boxes, counts);
+                                                                  L.boxes, L.counts);
     DNR_CHECK_LAUNCH();
     size_t temp = L.cub_bytes;
-    DNR_CUDA(cub::DeviceScan::InclusiveSum(base + L.cub_temp, temp, counts, scan, n_faces, s));
+    DNR_CUDA(cub::DeviceScan::InclusiveSum(L.cub_temp, temp, L.counts, L.scan, n_faces, s));
     depth_raster_kernel<<<DNR_NUM_SMS * 16, RASTER_THREADS, 0, s>>>(vertices, n_vertices, faces, n_faces, cam, width, near, far,
-                                                                    boxes, scan, zbuf + pixels * v);
+                                                                    L.boxes, L.scan, zbuf + pixels * v);
     DNR_CHECK_LAUNCH();
   }
   depth_resolve_kernel<<<DNR_NUM_SMS * 8, 256, 0, s>>>(zbuf, pixels * n_views);

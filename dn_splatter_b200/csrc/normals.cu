@@ -37,38 +37,34 @@ constexpr int CAP = 768;          // candidate buffer entries per warp (>= 2 * D
 constexpr int QWARPS = 2;         // warps per block of the query kernel (32 KB of static shared memory)
 constexpr int LEVEL_DIV = 2;      // scan cells of edge >= R / LEVEL_DIV
 
-__host__ size_t al256(size_t x) { return (x + 255) & ~size_t(255); }
-
 struct NrmLayout {
-  size_t keys_a, keys_b, vals_a, vals_b, scan, ustart, upts, ukey, umin, unormal, ucount, cub_temp, total, cub_bytes;
-  cudaError_t err;  // of cub's temp-size queries (they need a device: without one the scratch is sized 0)
+  DnrCarver carve;
+  uint64_t *keys_a, *keys_b, *ukey;
+  int32_t *vals_a, *vals_b, *scan, *ustart, *umin, *ucount;
+  double *upts, *unormal;
+  void* cub_temp;
+  size_t cub_bytes;
+  NrmLayout(void* base, int64_t n) : carve(base) {
+    const size_t N = (size_t)n;
+    keys_a = carve.take<uint64_t>(N);
+    keys_b = carve.take<uint64_t>(N);
+    vals_a = carve.take<int32_t>(N);
+    vals_b = carve.take<int32_t>(N);
+    scan = carve.take<int32_t>(N);
+    ustart = carve.take<int32_t>(N + 1);
+    upts = carve.take<double>(3 * N);
+    ukey = carve.take<uint64_t>(N);
+    umin = carve.take<int32_t>(N);
+    unormal = carve.take<double>(3 * N);
+    ucount = carve.take<int32_t>(N);
+    size_t t1 = 0, t2 = 0;
+    const cudaError_t e1 = cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint64_t*)nullptr, (uint64_t*)nullptr,
+                                                           (const int32_t*)nullptr, (int32_t*)nullptr, (int)n, 0, 64);
+    const cudaError_t e2 = cub::DeviceScan::InclusiveSum(nullptr, t2, (const int32_t*)nullptr, (int32_t*)nullptr, (int)n);
+    cub_bytes = t1 > t2 ? t1 : t2;
+    cub_temp = carve.cub_scratch(e1 != cudaSuccess ? e1 : e2, cub_bytes);
+  }
 };
-
-NrmLayout nrm_layout(int64_t n) {
-  NrmLayout L;
-  size_t off = 0;
-  const size_t N = (size_t)n;
-  L.keys_a = off; off = al256(off + 8 * N);
-  L.keys_b = off; off = al256(off + 8 * N);
-  L.vals_a = off; off = al256(off + 4 * N);
-  L.vals_b = off; off = al256(off + 4 * N);
-  L.scan = off; off = al256(off + 4 * N);
-  L.ustart = off; off = al256(off + 4 * (N + 1));
-  L.upts = off; off = al256(off + 24 * N);
-  L.ukey = off; off = al256(off + 8 * N);
-  L.umin = off; off = al256(off + 4 * N);
-  L.unormal = off; off = al256(off + 24 * N);
-  L.ucount = off; off = al256(off + 4 * N);
-  size_t t1 = 0, t2 = 0;
-  const cudaError_t e1 = cub::DeviceRadixSort::SortPairs(nullptr, t1, (const uint64_t*)nullptr, (uint64_t*)nullptr, (const int32_t*)nullptr,
-                                  (int32_t*)nullptr, (int)n, 0, 64);
-  const cudaError_t e2 = cub::DeviceScan::InclusiveSum(nullptr, t2, (const int32_t*)nullptr, (int32_t*)nullptr, (int)n);
-  L.err = e1 != cudaSuccess ? e1 : e2;
-  L.cub_bytes = t1 > t2 ? t1 : t2;
-  L.cub_temp = off; off = al256(off + L.cub_bytes);
-  L.total = off;
-  return L;
-}
 
 struct GridP {
   double lo[3], inv_cell;
@@ -603,7 +599,7 @@ extern "C" int dnr_dn_backproject(const float* depth, int32_t width, int32_t hei
 
 extern "C" int64_t dnr_dn_normals_workspace_bytes(int64_t n_points) {
   if (n_points <= 0 || n_points > INT32_MAX - 1) return DNR_E_SIZE;
-  return (int64_t)nrm_layout(n_points).total;
+  return (int64_t)NrmLayout(nullptr, n_points).carve.total();
 }
 
 extern "C" int dnr_dn_normals(const double* points, int64_t n_points, const DnrDnSearch* search, void* ws, int64_t ws_bytes,
@@ -613,17 +609,12 @@ extern "C" int dnr_dn_normals(const double* points, int64_t n_points, const DnrD
   if (n_points <= 0 || n_points > INT32_MAX - 1) return DNR_E_SIZE;
   if (search->k <= 0 || search->k > DNR_DN_MAX_K) return DNR_E_OPTION;
   if (!(search->cell > 0.0) || !(search->cell < INFINITY)) return DNR_E_SIZE;
-  const NrmLayout L = nrm_layout(n_points);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
-  if (L.err != cudaSuccess) return (int)L.err;  // the cub scratch could not be sized: never run without it
+  const NrmLayout L(ws, n_points);
+  if (const int e = L.carve.check(ws_bytes)) return e;
   const int n = (int)n_points;
   cudaStream_t s = (cudaStream_t)stream;
-  char* base = (char*)ws;
-  uint64_t* ka = (uint64_t*)(base + L.keys_a);
-  uint64_t* kb = (uint64_t*)(base + L.keys_b);
-  int32_t* va = (int32_t*)(base + L.vals_a);
-  int32_t* vb = (int32_t*)(base + L.vals_b);
-  int32_t* scan = (int32_t*)(base + L.scan);
+  uint64_t *ka = L.keys_a, *kb = L.keys_b;
+  int32_t *va = L.vals_a, *vb = L.vals_b, *scan = L.scan;
   GridP g;
   for (int a = 0; a < 3; ++a) g.lo[a] = search->lo[a];
   g.inv_cell = 1.0 / search->cell;
@@ -632,27 +623,23 @@ extern "C" int dnr_dn_normals(const double* points, int64_t n_points, const DnrD
     nrm_keys_kernel<<<blocks, 256, 0, s>>>(points, n, pass, g, va, ka, va);
     DNR_CHECK_LAUNCH();
     size_t temp = L.cub_bytes;
-    DNR_CUDA(cub::DeviceRadixSort::SortPairs(base + L.cub_temp, temp, ka, kb, va, vb, n, 0, pass < 3 ? 64 : 3 * MORTON_BITS, s));
+    DNR_CUDA(cub::DeviceRadixSort::SortPairs(L.cub_temp, temp, ka, kb, va, vb, n, 0, pass < 3 ? 64 : 3 * MORTON_BITS, s));
     DNR_CUDA(cudaMemcpyAsync(va, vb, 4 * (size_t)n, cudaMemcpyDeviceToDevice, s));
   }
   nrm_heads_kernel<<<blocks, 256, 0, s>>>(points, n, va, vb);
   DNR_CHECK_LAUNCH();
   size_t temp = L.cub_bytes;
-  DNR_CUDA(cub::DeviceScan::InclusiveSum(base + L.cub_temp, temp, vb, scan, n, s));
-  double* upts = (double*)(base + L.upts);
-  uint64_t* ukey = (uint64_t*)(base + L.ukey);
-  int32_t* umin = (int32_t*)(base + L.umin);
-  int32_t* ustart = (int32_t*)(base + L.ustart);
-  nrm_unique_kernel<<<blocks, 256, 0, s>>>(points, n, va, kb, scan, ustart, upts, ukey, umin);
+  DNR_CUDA(cub::DeviceScan::InclusiveSum(L.cub_temp, temp, vb, scan, n, s));
+  nrm_unique_kernel<<<blocks, 256, 0, s>>>(points, n, va, kb, scan, L.ustart, L.upts, L.ukey, L.umin);
   DNR_CHECK_LAUNCH();
   QueryArgs a;
-  a.upts = upts; a.ukey = ukey; a.umin = umin; a.ustart = ustart; a.order = va; a.n_unique = scan + (n - 1);
-  a.unormal = (double*)(base + L.unormal); a.ucount = (int32_t*)(base + L.ucount); a.cov = cov; a.nbr = neighbours; a.stats = stats; a.g = g; a.cell = search->cell;
+  a.upts = L.upts; a.ukey = L.ukey; a.umin = L.umin; a.ustart = L.ustart; a.order = va; a.n_unique = scan + (n - 1);
+  a.unormal = L.unormal; a.ucount = L.ucount; a.cov = cov; a.nbr = neighbours; a.stats = stats; a.g = g; a.cell = search->cell;
   for (int j = 0; j < 3; ++j) a.center[j] = search->center[j];
   a.orient = search->orient; a.k = search->k; a.n = n;
   nrm_query_kernel<<<(n + QWARPS - 1) / QWARPS, 32 * QWARPS, 0, s>>>(a);
   DNR_CHECK_LAUNCH();
-  nrm_scatter_kernel<<<blocks, 256, 0, s>>>(n, search->k, va, scan, ustart, a.unormal, a.ucount, normals, examined, cov, neighbours);
+  nrm_scatter_kernel<<<blocks, 256, 0, s>>>(n, search->k, va, scan, L.ustart, a.unormal, a.ucount, normals, examined, cov, neighbours);
   DNR_CHECK_LAUNCH();
   return 0;
 }

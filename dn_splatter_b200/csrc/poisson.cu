@@ -282,36 +282,34 @@ __global__ void __launch_bounds__(THREADS) color_kernel(int R, const int32_t* __
   out[4 * n + 3] = (float)w;
 }
 
-__host__ size_t align256(size_t x) { return (x + 255) & ~size_t(255); }
-
 struct SplatLayout {
-  size_t keys_in, keys_out, idx_in, idx_out, cub, cub_bytes, sf, sn, sc, start, count0, count1, part, sum, total;
+  DnrCarver carve;
+  uint32_t *keys_in, *keys_out;
+  int32_t *idx_in, *idx_out, *start;
+  void* cub_temp;
+  size_t cub_bytes = 0;
+  float4 *sf, *sn, *sc;
+  float *count0, *count1;
+  double *part, *sum;
+  SplatLayout(void* base, int depth, int64_t n) : carve(base) {
+    const int64_t R = 1ll << depth, N = R * R * R;
+    keys_in = carve.take<uint32_t>(n);
+    keys_out = carve.take<uint32_t>(n);
+    idx_in = carve.take<int32_t>(n);
+    idx_out = carve.take<int32_t>(n);
+    const cudaError_t e = cub::DeviceRadixSort::SortPairs(nullptr, cub_bytes, (const uint32_t*)nullptr, (uint32_t*)nullptr,
+                                                          (const int32_t*)nullptr, (int32_t*)nullptr, (int)n, 0, 3 * depth);
+    cub_temp = carve.cub_scratch(e, cub_bytes);
+    sf = carve.take<float4>(n);
+    sn = carve.take<float4>(n);
+    sc = carve.take<float4>(n);
+    start = carve.take<int32_t>(N + 1);
+    count0 = carve.take<float>(N);
+    count1 = carve.take<float>(N / 8);
+    part = carve.take<double>(RED_BLOCKS);
+    sum = carve.take<double>(1);
+  }
 };
-
-SplatLayout splat_layout(int depth, int64_t n) {
-  SplatLayout L;
-  const int64_t R = 1ll << depth, N = R * R * R;
-  size_t o = 0;
-  L.keys_in = o; o = align256(o + 4 * (size_t)n);
-  L.keys_out = o; o = align256(o + 4 * (size_t)n);
-  L.idx_in = o; o = align256(o + 4 * (size_t)n);
-  L.idx_out = o; o = align256(o + 4 * (size_t)n);
-  size_t temp = 0;
-  cub::DeviceRadixSort::SortPairs(nullptr, temp, (const uint32_t*)nullptr, (uint32_t*)nullptr, (const int32_t*)nullptr,
-                                  (int32_t*)nullptr, (int)n, 0, 3 * depth);
-  L.cub_bytes = temp;
-  L.cub = o; o = align256(o + temp);
-  L.sf = o; o = align256(o + 16 * (size_t)n);
-  L.sn = o; o = align256(o + 16 * (size_t)n);
-  L.sc = o; o = align256(o + 16 * (size_t)n);
-  L.start = o; o = align256(o + 4 * (size_t)(N + 1));
-  L.count0 = o; o = align256(o + 4 * (size_t)N);
-  L.count1 = o; o = align256(o + 4 * (size_t)(N / 8));
-  L.part = o; o = align256(o + 8 * (size_t)RED_BLOCKS);
-  L.sum = o; o = align256(o + 8);
-  L.total = o;
-  return L;
-}
 
 int check_grid(const DnrPoissonGrid* g, Geo* geo) {
   if (!g) return DNR_E_NULL;
@@ -492,25 +490,23 @@ __global__ void subtract_mean_kernel(float* __restrict__ x, int64_t N, const dou
 }
 
 struct SolveLayout {
-  size_t b0, lvl[DNR_POISSON_MAX_DEPTH][3], part, hist, total;  // lvl[l] = {x, b, S} for l >= 1
-  int levels;                                                   // number of levels incl. the finest
-};
-
-SolveLayout solve_layout(int depth, int max_cycles) {
-  SolveLayout L;
-  size_t o = 0;
-  const int64_t R = 1ll << depth;
-  L.b0 = o; o = align256(o + 4 * (size_t)(R * R * R));
-  L.levels = depth - 1;  // down to 4^3
-  for (int l = 1; l < L.levels; ++l) {
-    const int64_t Rl = R >> l, Nl = Rl * Rl * Rl;
-    for (int q = 0; q < 3; ++q) { L.lvl[l][q] = o; o = align256(o + 4 * (size_t)Nl); }
+  DnrCarver carve;
+  float* b0;
+  float* lvl[DNR_POISSON_MAX_DEPTH][3];  // lvl[l] = {x, b, S} for l >= 1
+  double *part, *hist;
+  int levels;  // number of levels incl. the finest
+  SolveLayout(void* base, int depth, int max_cycles) : carve(base) {
+    const int64_t R = 1ll << depth;
+    b0 = carve.take<float>(R * R * R);
+    levels = depth - 1;  // down to 4^3
+    for (int l = 1; l < levels; ++l) {
+      const int64_t Rl = R >> l, Nl = Rl * Rl * Rl;
+      for (int q = 0; q < 3; ++q) lvl[l][q] = carve.take<float>(Nl);
+    }
+    part = carve.take<double>(RED_BLOCKS);
+    hist = carve.take<double>(max_cycles + 2);
   }
-  L.part = o; o = align256(o + 8 * (size_t)RED_BLOCKS);
-  L.hist = o; o = align256(o + 8 * (size_t)(max_cycles + 2));
-  L.total = o;
-  return L;
-}
+};
 
 unsigned red_blocks(int64_t N) { return (unsigned)std::min<int64_t>(RED_BLOCKS, (N + THREADS - 1) / THREADS); }
 
@@ -595,7 +591,7 @@ extern "C" int64_t dnr_poisson_splat_workspace_bytes(const DnrPoissonGrid* grid,
   const int rc = check_grid(grid, &g);
   if (rc) return rc;
   if (n_points <= 0 || n_points > INT32_MAX) return DNR_E_SIZE;
-  return (int64_t)splat_layout(g.depth, n_points).total;
+  return (int64_t)SplatLayout(nullptr, g.depth, n_points).carve.total();
 }
 
 extern "C" int dnr_poisson_splat(const DnrPoissonGrid* grid, const float* points, const float* normals, const float* colors,
@@ -607,29 +603,21 @@ extern "C" int dnr_poisson_splat(const DnrPoissonGrid* grid, const float* points
   if (n_points <= 0 || n_points > INT32_MAX) return DNR_E_SIZE;
   if (!points || !normals || !ws || !screen || !faces || !density || !area_scale) return DNR_E_NULL;
   if ((colors == nullptr) != (color_grid == nullptr)) return DNR_E_NULL;
-  const SplatLayout L = splat_layout(g.depth, n_points);
-  if ((int64_t)L.total > ws_bytes) return DNR_E_WORKSPACE;
+  const SplatLayout L(ws, g.depth, n_points);
+  if (const int e = L.carve.check(ws_bytes)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  char* w = (char*)ws;
   const int n = (int)n_points, R = g.R;
   const int64_t N = (int64_t)R * R * R;
-  uint32_t* keys_in = (uint32_t*)(w + L.keys_in);
-  uint32_t* keys = (uint32_t*)(w + L.keys_out);
-  int32_t* idx_in = (int32_t*)(w + L.idx_in);
-  int32_t* order = (int32_t*)(w + L.idx_out);
-  float4* sf = (float4*)(w + L.sf);
-  float4* sn = (float4*)(w + L.sn);
-  float4* sc = (float4*)(w + L.sc);
-  int32_t* start = (int32_t*)(w + L.start);
-  float* count0 = (float*)(w + L.count0);
-  float* count1 = (float*)(w + L.count1);
-  double* part = (double*)(w + L.part);
-  double* sum = (double*)(w + L.sum);
+  uint32_t *keys_in = L.keys_in, *keys = L.keys_out;
+  int32_t *idx_in = L.idx_in, *order = L.idx_out, *start = L.start;
+  float4 *sf = L.sf, *sn = L.sn, *sc = L.sc;
+  float *count0 = L.count0, *count1 = L.count1;
+  double *part = L.part, *sum = L.sum;
 
   keys_kernel<<<blocks_for(n), THREADS, 0, s>>>(g, points, n, keys_in, idx_in);
   DNR_CHECK_LAUNCH();
   size_t temp = L.cub_bytes;
-  DNR_CUDA(cub::DeviceRadixSort::SortPairs(w + L.cub, temp, keys_in, keys, idx_in, order, n, 0, 3 * g.depth, s));
+  DNR_CUDA(cub::DeviceRadixSort::SortPairs(L.cub_temp, temp, keys_in, keys, idx_in, order, n, 0, 3 * g.depth, s));
   gather_kernel<<<blocks_for(n), THREADS, 0, s>>>(g, points, normals, colors, order, n, sf, sn, sc);
   DNR_CHECK_LAUNCH();
   cell_start_kernel<<<blocks_for(N + 1), THREADS, 0, s>>>(keys, n, N, start);
@@ -663,7 +651,7 @@ extern "C" int64_t dnr_poisson_solve_workspace_bytes(const DnrPoissonGrid* grid,
   const int rc = check_grid(grid, &g);
   if (rc) return rc;
   if (max_cycles < 1 || max_cycles > DNR_POISSON_MAX_CYCLES) return DNR_E_SIZE;
-  return (int64_t)solve_layout(g.depth, max_cycles).total;
+  return (int64_t)SolveLayout(nullptr, g.depth, max_cycles).carve.total();
 }
 
 extern "C" int dnr_poisson_solve(const DnrPoissonGrid* grid, const float* screen, const float* faces, float screen_weight,
@@ -675,18 +663,15 @@ extern "C" int dnr_poisson_solve(const DnrPoissonGrid* grid, const float* screen
   if (max_cycles < 1 || max_cycles > DNR_POISSON_MAX_CYCLES) return DNR_E_SIZE;
   if (!(screen_weight >= 0.f) || !(tol >= 0.f)) return DNR_E_SIZE;
   if (!screen || !faces || !ws || !chi || !residual_host || !cycles_host) return DNR_E_NULL;
-  const SolveLayout SL = solve_layout(g.depth, max_cycles);
-  if ((int64_t)SL.total > ws_bytes) return DNR_E_WORKSPACE;
+  const SolveLayout SL(ws, g.depth, max_cycles);
+  if (const int e = SL.carve.check(ws_bytes)) return e;
   cudaStream_t s = (cudaStream_t)stream;
-  char* w = (char*)ws;
   const int R = g.R;
   const int64_t N = (int64_t)R * R * R;
   Level lv[DNR_POISSON_MAX_DEPTH];
-  lv[0] = Level{R, 1.f, chi, (float*)(w + SL.b0), screen};
-  for (int l = 1; l < SL.levels; ++l)
-    lv[l] = Level{R >> l, (float)(1 << l), (float*)(w + SL.lvl[l][0]), (float*)(w + SL.lvl[l][1]), (const float*)(w + SL.lvl[l][2])};
-  double* part = (double*)(w + SL.part);
-  double* hist = (double*)(w + SL.hist);  // [0] = ||b||^2, [c] = ||r||^2 after cycle c
+  lv[0] = Level{R, 1.f, chi, SL.b0, screen};
+  for (int l = 1; l < SL.levels; ++l) lv[l] = Level{R >> l, (float)(1 << l), SL.lvl[l][0], SL.lvl[l][1], SL.lvl[l][2]};
+  double *part = SL.part, *hist = SL.hist;  // hist[0] = ||b||^2, [c] = ||r||^2 after cycle c
 
   rhs_kernel<<<blocks_for(N), THREADS, 0, s>>>(R, faces, lv[0].b);
   DNR_CHECK_LAUNCH();

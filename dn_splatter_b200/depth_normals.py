@@ -33,7 +33,6 @@ import numpy as np
 import torch
 
 from . import _lib as L
-from .sugar import _need_cuda, _stream
 
 SCALE_FACTOR = 0.001
 OPENGL_TO_OPENCV = np.diag([1.0, -1.0, -1.0, 1.0])
@@ -134,7 +133,7 @@ def backproject_depth(depth, fx, fy, cx, cy, c2w: np.ndarray, with_camera: bool 
     """World points [h*w,3] f64 (device) of a depth frame [h,w] in metres, as the scripts' backproject forms them; with
     with_camera also the f32 camera coordinates [h*w,3]."""
     d = torch.as_tensor(depth, dtype=torch.float32, device="cuda").contiguous()
-    _need_cuda(d)
+    L.need_cuda(d)
     h, w = d.shape
     if not bool(torch.isfinite(d).all()):
         raise ValueError("backproject_depth: the depth map holds non-finite values")
@@ -144,16 +143,14 @@ def backproject_depth(depth, fx, fy, cx, cy, c2w: np.ndarray, with_camera: bool 
     c2w = np.asarray(c2w, np.float64)
     pose = _pose(np.linalg.inv(c2w[:3, :3]), c2w[:3, 3])
     L.check(L.load().dnr_dn_backproject(d.data_ptr(), w, h, intr, C.byref(pose), None if cam is None else cam.data_ptr(),
-                                        pts.data_ptr(), _stream()), "dnr_dn_backproject")
+                                        pts.data_ptr(), L.stream()), "dnr_dn_backproject")
     return (pts, cam) if with_camera else pts
 
 
 def required_bytes(n_points: int) -> int:
     """Device bytes of one estimate_normals call on n points: the search workspace, the points and the normals, plus the
     frame, mono image, angle and encoded outputs of a consistency pass."""
-    ws = int(L.load().dnr_dn_normals_workspace_bytes(int(n_points)))
-    if ws < 0:
-        L.check(ws, "dnr_dn_normals_workspace_bytes")
+    ws = L.workspace_bytes(L.load().dnr_dn_normals_workspace_bytes, int(n_points))
     return ws + n_points * (24 + 24 + 4 + 3 + 8 + 1 + 3)
 
 
@@ -177,7 +174,7 @@ def estimate_normals(points, knn: int = KNN, center=None, *, intrinsics=None, c2
         points = backproject_depth(points, *intrinsics, c2w)
         center = np.asarray(c2w, np.float64)[:3, 3]
     pts = torch.as_tensor(points, device="cuda").to(torch.float64).contiguous()
-    _need_cuda(pts)
+    L.need_cuda(pts)
     if pts.ndim != 2 or pts.shape[1] != 3 or pts.shape[0] == 0:
         raise ValueError(f"estimate_normals: points must be [N,3] with N > 0, got {tuple(pts.shape)}")
     if not 1 <= knn <= L.DN_MAX_K:
@@ -195,10 +192,7 @@ def estimate_normals(points, knn: int = KNN, center=None, *, intrinsics=None, c2
     s.center[:] = [0.0, 0.0, 0.0] if center is None else np.asarray(center, np.float64).tolist()
     s.k, s.orient = int(knn), int(center is not None)
     lib = L.load()
-    nbytes = int(lib.dnr_dn_normals_workspace_bytes(n))
-    if nbytes < 0:
-        L.check(nbytes, "dnr_dn_normals_workspace_bytes")
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=pts.device)
+    ws, nbytes = L.workspace(lib.dnr_dn_normals_workspace_bytes, n, device=pts.device)
     normals = torch.empty((n, 3), dtype=torch.float64, device=pts.device)
     cov = torch.empty((n, 9), dtype=torch.float64, device=pts.device) if debug else None
     nbr = torch.empty((n, knn), dtype=torch.int32, device=pts.device) if debug else None
@@ -206,7 +200,7 @@ def estimate_normals(points, knn: int = KNN, center=None, *, intrinsics=None, c2
         raise ValueError("estimate_normals: examined must be a contiguous int32 tensor of N elements")
     L.check(lib.dnr_dn_normals(pts.data_ptr(), n, C.byref(s), ws.data_ptr(), nbytes, normals.data_ptr(),
                                None if examined is None else examined.data_ptr(), None if cov is None else cov.data_ptr(), None if nbr is None else nbr.data_ptr(),
-                               None if stats is None else stats.data_ptr(), _stream()), "dnr_dn_normals")
+                               None if stats is None else stats.data_ptr(), L.stream()), "dnr_dn_normals")
     return (normals, cov, nbr) if debug else normals
 
 
@@ -227,7 +221,7 @@ def depth_normal_consistency(normals, mono_u8, c2w: np.ndarray, mode: str = "omn
     enc = torch.empty((n, 3), dtype=torch.uint8, device=nrm.device)
     rot = _pose(np.transpose(np.linalg.inv(np.asarray(c2w, np.float64))[:3, :3]))
     L.check(L.load().dnr_dn_consistency(nrm.data_ptr(), mono.data_ptr(), n, C.byref(rot), MODES[mode], float(threshold),
-                                        deg.data_ptr(), mask.data_ptr(), enc.data_ptr(), _stream()), "dnr_dn_consistency")
+                                        deg.data_ptr(), mask.data_ptr(), enc.data_ptr(), L.stream()), "dnr_dn_consistency")
     return enc, deg, mask
 
 

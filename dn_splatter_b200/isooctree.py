@@ -33,7 +33,6 @@ from torch import Tensor
 
 from . import _lib as L
 from .mesh import TriangleMesh, marching_cubes, write_obj, write_ply
-from .sugar import _need_cuda, _stream
 
 CAM_CONVENTION_CHANGE = np.diag([1.0, -1.0, -1.0, 1.0])
 DEPTH_SCALE = 1 / 1000.0  # the depth files hold millimetres
@@ -119,7 +118,7 @@ class FrameSet:
         self.normals = torch.zeros((n_frames, h, w, 3), dtype=torch.float32, device=device)
         self._poses = np.zeros((n_frames, L.ISO_POSE), np.float64)
         self.poses = None
-        _need_cuda(self.depth)
+        L.need_cuda(self.depth)
 
     @property
     def n_frames(self) -> int:
@@ -163,28 +162,20 @@ class FrameSet:
         return s
 
 
-def _ws_bytes(fn, *args) -> int:
-    n = int(fn(*args))
-    if n < 0:
-        L.check(n, "workspace query")
-    return n
-
-
 def hint_samples(fs: FrameSet, pixel_stride: int, with_normals: bool = False):
     """(points [n,3] f64, normals [n,3] f64 or None): Frame.get_samples(stride=pixel_stride) of every frame, stacked in
     frame order.  One host read."""
     lib = L.load()
     s = fs.struct()
-    nbytes = _ws_bytes(lib.dnr_iso_samples_workspace_bytes, C.byref(s), int(pixel_stride))
     w, h = fs.camera.resolution
     cap = fs.n_frames * (-(-h // pixel_stride)) * (-(-w // pixel_stride))
     dev = fs.depth.device
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    ws, nbytes = L.workspace(lib.dnr_iso_samples_workspace_bytes, C.byref(s), int(pixel_stride), device=dev)
     pts = torch.empty((cap, 3), dtype=torch.float64, device=dev)
     nrm = torch.empty((cap, 3), dtype=torch.float64, device=dev) if with_normals else None
     count = C.c_int64()
     L.check(lib.dnr_iso_samples(C.byref(s), int(pixel_stride), ws.data_ptr(), nbytes, pts.data_ptr(),
-                                None if nrm is None else nrm.data_ptr(), C.byref(count), _stream()), "dnr_iso_samples")
+                                None if nrm is None else nrm.data_ptr(), C.byref(count), L.stream()), "dnr_iso_samples")
     n = count.value
     return pts[:n], (None if nrm is None else nrm[:n])
 
@@ -228,7 +219,7 @@ def iso_grid(origin, side: float, max_depth: int, subdivision_threshold: int) ->
 
 def build_octree(hint: Tensor, max_depth: int, subdivision_threshold: int) -> Octree:
     """The octree of the hint cloud [n,3] f64 (device), its leaves and their unique corners.  One host read per level."""
-    _need_cuda(hint)
+    L.need_cuda(hint)
     if hint.shape[0] == 0:
         raise ValueError("isooctree: the hint cloud is empty (no depth sample survived the validity tests)")
     lib = L.load()
@@ -236,20 +227,18 @@ def build_octree(hint: Tensor, max_depth: int, subdivision_threshold: int) -> Oc
     origin, side = root_cube(h)
     g = iso_grid(origin, side, max_depth, subdivision_threshold)
     dev = h.device
-    nbytes = _ws_bytes(lib.dnr_iso_octree_workspace_bytes, C.byref(g), h.shape[0])
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    ws, nbytes = L.workspace(lib.dnr_iso_octree_workspace_bytes, C.byref(g), h.shape[0], device=dev)
     counts = (C.c_int64 * (max_depth + 1))()
-    L.check(lib.dnr_iso_octree(C.byref(g), h.data_ptr(), h.shape[0], ws.data_ptr(), nbytes, counts, _stream()), "dnr_iso_octree")
+    L.check(lib.dnr_iso_octree(C.byref(g), h.data_ptr(), h.shape[0], ws.data_ptr(), nbytes, counts, L.stream()), "dnr_iso_octree")
     n_leaves = sum(counts)
-    cbytes = _ws_bytes(lib.dnr_iso_corners_workspace_bytes, C.byref(g), n_leaves)
-    ws2 = torch.empty(cbytes, dtype=torch.uint8, device=dev)
+    ws2, cbytes = L.workspace(lib.dnr_iso_corners_workspace_bytes, C.byref(g), n_leaves, device=dev)
     leaves = torch.empty(n_leaves, dtype=torch.int64, device=dev)
     keys = torch.empty(8 * n_leaves, dtype=torch.int64, device=dev)
     pts = torch.empty((8 * n_leaves, 3), dtype=torch.float64, device=dev)
     lc = torch.empty((n_leaves, 8), dtype=torch.int32, device=dev)
     n_corners = C.c_int64()
     L.check(lib.dnr_iso_corners(C.byref(g), ws.data_ptr(), counts, ws2.data_ptr(), cbytes, leaves.data_ptr(), keys.data_ptr(),
-                                pts.data_ptr(), lc.data_ptr(), C.byref(n_corners), _stream()), "dnr_iso_corners")
+                                pts.data_ptr(), lc.data_ptr(), C.byref(n_corners), L.stream()), "dnr_iso_corners")
     n = n_corners.value
     return Octree(g, leaves, tuple(int(c) for c in counts), keys[:n], pts[:n], lc)
 
@@ -258,7 +247,7 @@ def iso_eval(fs: FrameSet, points: Tensor, max_tsdf_rel: float = 0.05, max_angle
              max_tsdf_abs: Optional[float] = None, choose_best_frame: bool = False, two_pass: bool = True,
              use_normals: bool = True) -> Tensor:
     """isoFunc of build_mesh_projection at points [n,3] (device): values [n] f32.  No host read."""
-    _need_cuda(points)
+    L.need_cuda(points)
     if not use_normals:
         choose_best_frame, two_pass = False, False
     p = L.DnrIsoParams()
@@ -269,7 +258,7 @@ def iso_eval(fs: FrameSet, points: Tensor, max_tsdf_rel: float = 0.05, max_angle
     p.passes = 1 if choose_best_frame else (3 if two_pass else 2)
     pts = points.detach().to(torch.float64).contiguous()
     out = torch.empty(pts.shape[0], dtype=torch.float32, device=pts.device)
-    L.check(L.load().dnr_iso_eval(C.byref(fs.struct()), C.byref(p), pts.data_ptr(), pts.shape[0], out.data_ptr(), _stream()),
+    L.check(L.load().dnr_iso_eval(C.byref(fs.struct()), C.byref(p), pts.data_ptr(), pts.shape[0], out.data_ptr(), L.stream()),
             "dnr_iso_eval")
     return out
 
@@ -281,7 +270,7 @@ def fill_grid(tree: Octree, corner_values: Tensor) -> Tensor:
     field = torch.empty((R1, R1, R1), dtype=torch.float32, device=v.device)
     counts = (C.c_int64 * len(tree.level_counts))(*tree.level_counts)
     L.check(L.load().dnr_iso_fill(C.byref(tree.grid), tree.leaves.data_ptr(), counts, tree.leaf_corners.data_ptr(), v.data_ptr(),
-                                  field.data_ptr(), _stream()), "dnr_iso_fill")
+                                  field.data_ptr(), L.stream()), "dnr_iso_fill")
     return field
 
 
@@ -294,17 +283,17 @@ def required_bytes(n_frames: int, width: int, height: int, pixel_stride: int, ma
     frames = n_frames * width * height * 16 + n_frames * L.ISO_POSE * 8
     hint = cand * (24 + 9) + 4096
     g = iso_grid((0.0, 0.0, 0.0), 1.0, max_depth, subdivision_threshold)
-    octree = _ws_bytes(lib.dnr_iso_octree_workspace_bytes, C.byref(g), cand)
+    octree = L.workspace_bytes(lib.dnr_iso_octree_workspace_bytes, C.byref(g), cand)
     by_count, bound, pw = cand // subdivision_threshold, 1, 1
     for _ in range(1, max_depth):
         pw *= 8
         bound = max(bound, min(pw, by_count))
     n_leaves = max_depth * 8 * bound + 1
-    corners = _ws_bytes(lib.dnr_iso_corners_workspace_bytes, C.byref(g), n_leaves) + n_leaves * (8 + 8 * (8 + 24 + 4))
+    corners = L.workspace_bytes(lib.dnr_iso_corners_workspace_bytes, C.byref(g), n_leaves) + n_leaves * (8 + 8 * (8 + 24 + 4))
     R1 = (1 << max_depth) + 1
     mc = L.DnrMcField()
     mc.values, mc.dims[0], mc.dims[1], mc.dims[2], mc.spacing = 1, R1, R1, R1, 1.0
-    field = 4 * R1 ** 3 + _ws_bytes(lib.dnr_mc_count_workspace_bytes, C.byref(mc))
+    field = 4 * R1 ** 3 + L.workspace_bytes(lib.dnr_mc_count_workspace_bytes, C.byref(mc))
     return frames + hint + octree + corners + field
 
 

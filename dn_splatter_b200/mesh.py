@@ -23,7 +23,7 @@ import torch
 from torch import Tensor
 
 from . import _lib as L
-from .sugar import KNN, KnnIndex, _need_cuda, _stream, get_closest_gaussians, get_density
+from .sugar import KNN, KnnIndex, get_closest_gaussians, get_density
 
 VOXEL_BYTES = 16
 TSDF_MESH_NAME = "Open3dTSDFfusion_mesh.ply"
@@ -47,17 +47,11 @@ def snap_bounds(bounds, voxel_size: float):
 
 def _mc(field: "L.DnrMcField", device, with_colors: bool) -> TriangleMesh:
     lib = L.load()
-    nbytes = lib.dnr_mc_count_workspace_bytes(C.byref(field))
-    if nbytes < 0:
-        L.check(int(nbytes), "dnr_mc_count_workspace_bytes")
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=device)
+    ws, nbytes = L.workspace(lib.dnr_mc_count_workspace_bytes, C.byref(field), device=device)
     counts = (C.c_int64 * 3)()
-    L.check(lib.dnr_mc_count(C.byref(field), ws.data_ptr(), nbytes, counts, _stream()), "dnr_mc_count")
+    L.check(lib.dnr_mc_count(C.byref(field), ws.data_ptr(), nbytes, counts, L.stream()), "dnr_mc_count")
     n_faces, n_verts = int(counts[1]), int(counts[2])
-    ebytes = lib.dnr_mc_emit_workspace_bytes(counts)
-    if ebytes < 0:
-        L.check(int(ebytes), "dnr_mc_emit_workspace_bytes")
-    ws2 = torch.empty(max(ebytes, 1), dtype=torch.uint8, device=device)
+    ws2, ebytes = L.workspace(lib.dnr_mc_emit_workspace_bytes, counts, device=device)
     verts = torch.empty((n_verts, 3), dtype=torch.float32, device=device)
     faces = torch.empty((n_faces, 3), dtype=torch.int32, device=device)
     colors = torch.empty((n_verts, 3), dtype=torch.float32, device=device) if with_colors else None
@@ -66,7 +60,7 @@ def _mc(field: "L.DnrMcField", device, with_colors: bool) -> TriangleMesh:
         return t.data_ptr() if t is not None and t.numel() else None
 
     L.check(lib.dnr_mc_emit(C.byref(field), ws.data_ptr(), counts, ws2.data_ptr(), ebytes, ptr(verts), ptr(faces), ptr(colors),
-                            _stream()), "dnr_mc_emit")
+                            L.stream()), "dnr_mc_emit")
     return TriangleMesh(verts, faces, colors)
 
 
@@ -75,14 +69,14 @@ def marching_cubes(field: Tensor, iso: float, origin: Sequence[float], spacing: 
     """Marching cubes on the device over field [X,Y,Z] sampled at origin + (i, j, k) * spacing.  Inside is field < iso;
     cubes with a corner where valid == 0 emit nothing.  Vertices are welded and ordered by (sample index, edge axis),
     faces by cube index; the mesh has no colours.  One host read of the output sizes."""
-    _need_cuda(field)
+    L.need_cuda(field)
     f = field.detach().float().contiguous()
     if f.dim() != 3:
         raise ValueError(f"marching_cubes: field must be [X,Y,Z], got {tuple(f.shape)}")
     s = L.DnrMcField()
     s.values = f.data_ptr()
     if valid is not None:
-        _need_cuda(valid)
+        L.need_cuda(valid)
         v = valid.detach().reshape(f.shape).to(torch.uint8).contiguous()
         s.valid = v.data_ptr()
     s.dims[0], s.dims[1], s.dims[2] = f.shape
@@ -108,7 +102,7 @@ class TSDFVolume:
                              "voxel_size or tighter bounds")
         self.voxel_size, self.sdf_trunc, self.depth_trunc = float(voxel_size), float(sdf_trunc), float(depth_trunc)
         self.voxels = torch.zeros((n, 4), dtype=torch.float32, device=device)  # {tsdf, weight, fixed-point rgb as 64 bits}
-        _need_cuda(self.voxels)
+        L.need_cuda(self.voxels)
         g = self._grid = L.DnrTsdfGrid()
         g.origin[0], g.origin[1], g.origin[2] = self.origin
         g.voxel, g.sdf_trunc = self.voxel_size, self.sdf_trunc
@@ -128,16 +122,16 @@ class TSDFVolume:
         """Fuses one view: depth [H,W,1] (or [H,W]) and rgb [H,W,3] device maps, as the model renders them, and one
         Cameras view; mask [H,W] (or [H,W,1]) marks the pixels whose depth is used.  Enqueued on the current stream,
         no synchronisation (the camera pose is read on the host)."""
-        _need_cuda(depth, rgb)
+        L.need_cuda(depth, rgb)
         H, W = depth.shape[0], depth.shape[1]
         d = depth.detach().reshape(H, W).float().contiguous()
         c = rgb.detach().reshape(H, W, 3).float().contiguous()
         m = None
         if mask is not None:
-            _need_cuda(mask)
+            L.need_cuda(mask)
             m = mask.detach().reshape(H, W).to(torch.uint8).contiguous()
         L.check(L.load().dnr_tsdf_integrate(C.byref(self._grid), d.data_ptr(), c.data_ptr(), None if m is None else m.data_ptr(),
-                                             W, H, self.camera_block(camera), self.depth_trunc, _stream()),
+                                             W, H, self.camera_block(camera), self.depth_trunc, L.stream()),
                 "dnr_tsdf_integrate")
 
     def extract_mesh(self) -> TriangleMesh:

@@ -26,7 +26,7 @@ from torch import Tensor
 
 from . import _lib as L
 from .mesh import TriangleMesh, _quantile_sorted, _views, write_ply
-from .sugar import KnnIndex, _stream
+from .sugar import KnnIndex
 
 log = logging.getLogger(__name__)
 
@@ -76,12 +76,9 @@ def _depth_call(v: Tensor, f32: Tensor, cams: Tensor, W: int, H: int, near: floa
     if f32.shape[0] == 0:
         return out.zero_()
     lib = L.load()
-    nbytes = lib.dnr_mesh_depth_workspace_bytes(f32.shape[0])
-    if nbytes < 0:
-        L.check(int(nbytes), "dnr_mesh_depth_workspace_bytes")
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=v.device)
+    ws, nbytes = L.workspace(lib.dnr_mesh_depth_workspace_bytes, f32.shape[0], device=v.device)
     L.check(lib.dnr_mesh_depth(v.data_ptr(), v.shape[0], f32.data_ptr(), f32.shape[0], cams.data_ptr(), n, W, H, float(near),
-                               float(far), ws.data_ptr(), nbytes, out.data_ptr(), _stream()), "dnr_mesh_depth")
+                               float(far), ws.data_ptr(), nbytes, out.data_ptr(), L.stream()), "dnr_mesh_depth")
     return out
 
 
@@ -172,7 +169,7 @@ def visibility_counts(points: Tensor, cameras, rendered: Optional[Tensor] = None
             g = torch.stack([torch.as_tensor(gts[k]).to(device=dev, dtype=torch.float32).reshape(H, W) for k in range(c0, c1)])
         L.check(L.load().dnr_mesh_visibility(p.data_ptr(), p.shape[0], cams[c0:c1].contiguous().data_ptr(),
                                              None if r is None else r.data_ptr(), None if g is None else g.data_ptr(), c1 - c0,
-                                             W, H, float(eps), obs.data_ptr(), inv.data_ptr(), _stream()), "dnr_mesh_visibility")
+                                             W, H, float(eps), obs.data_ptr(), inv.data_ptr(), L.stream()), "dnr_mesh_visibility")
     return obs, inv
 
 

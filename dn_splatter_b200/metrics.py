@@ -23,7 +23,6 @@ Semantics (the reference's, torchmetrics' where it delegates):
 """
 from __future__ import annotations
 
-import ctypes as C
 from typing import Callable, Optional, Sequence, Tuple
 
 import torch
@@ -63,10 +62,6 @@ def tf_resize(img: Tensor, size: Sequence[int]) -> Tensor:
 
 
 # ---------------------------------------------------------------------------------------------------------- kernels
-def _stream():
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _channels_last(t: Tensor) -> Tensor:
     """[B,C,H,W] -> contiguous [B,H,W,C]; free for a view of channels-last images."""
     return t.permute(0, 2, 3, 1).contiguous()
@@ -89,7 +84,7 @@ def rgb_sums(pred: Tensor, gt: Tensor) -> Tensor:
     p, g, u8 = _pred_target(pred, gt)
     B, H, W, Cn = p.shape
     out = torch.empty((B, 2), dtype=torch.float64, device=p.device)
-    L.check(L.load().dnr_rgb_metrics(p.data_ptr(), g.data_ptr(), u8, B, H, W, Cn, out.data_ptr(), _stream()),
+    L.check(L.load().dnr_rgb_metrics(p.data_ptr(), g.data_ptr(), u8, B, H, W, Cn, out.data_ptr(), L.stream()),
             "dnr_rgb_metrics")
     return out.cpu()
 
@@ -104,7 +99,7 @@ def depth_sums(pred: Tensor, gt: Tensor, tolerance: float) -> Tensor:
         raise ValueError(f"pred is on {pred.device}, gt on {gt.device}")
     p, g = pred.float().contiguous(), gt.float().contiguous()
     out = torch.empty(9, dtype=torch.float64, device=p.device)
-    L.check(L.load().dnr_depth_metrics(p.data_ptr(), g.data_ptr(), p.numel(), float(tolerance), out.data_ptr(), _stream()),
+    L.check(L.load().dnr_depth_metrics(p.data_ptr(), g.data_ptr(), p.numel(), float(tolerance), out.data_ptr(), L.stream()),
             "dnr_depth_metrics")
     return out.cpu()
 
@@ -118,11 +113,10 @@ def normal_sums(pred: Tensor, gt: Tensor) -> Tensor:
     if Cn != 3:
         raise ValueError(f"normal maps have 3 channels, got {Cn}")
     lib = L.load()
-    ws_bytes = int(lib.dnr_normal_metrics_workspace_bytes(B, H, W))
-    ws = torch.empty(ws_bytes, dtype=torch.uint8, device=p.device)
+    ws, ws_bytes = L.workspace(lib.dnr_normal_metrics_workspace_bytes, B, H, W, device=p.device)
     out = torch.empty(3 * B + 1, dtype=torch.float64, device=p.device)
     L.check(lib.dnr_normal_metrics(p.data_ptr(), g.data_ptr(), u8, B, H, W, ws.data_ptr(), ws_bytes, out.data_ptr(),
-                                   _stream()), "dnr_normal_metrics")
+                                   L.stream()), "dnr_normal_metrics")
     return out.cpu()
 
 

@@ -97,7 +97,7 @@ class FusedAdam(torch.optim.Optimizer):
             assert p.dtype == g.dtype == torch.float32
             arr[i].p, arr[i].g, arr[i].m, arr[i].v = p.data_ptr(), g.data_ptr(), m.data_ptr(), v.data_ptr()
             arr[i].n, arr[i].lr, arr[i].eps, arr[i].bc1, arr[i].bc2_sqrt = p.numel(), lr, eps, bc1, bc2s
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        stream = L.stream()
         L.check(_timed("adam", L.load().dnr_adam_step, ctypes.cast(arr, ctypes.c_void_p), len(segs), b1, b2, stream),
                 "dnr_adam_step")
         return loss
@@ -148,7 +148,7 @@ class FusedAdam(torch.optim.Optimizer):
             arr[i].n, arr[i].lr, arr[i].eps, arr[i].bc1, arr[i].bc2_sqrt = p.numel(), lr, eps, bc1, bc2s
             widths[i] = p.numel() // bucket.n_gauss
             arr[i].dense = int(any(bucket.params[name] is p for name in bucket.dense_params))
-        stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+        stream = L.stream()
         L.check(L.load().dnr_adam_step_reduce(ctypes.cast(arr, ctypes.c_void_p), ctypes.cast(widths, ctypes.c_void_p), len(segs),
                                               b1, b2, ctypes.byref(pr), stream), "dnr_adam_step_reduce")
 

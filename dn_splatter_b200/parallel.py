@@ -77,7 +77,7 @@ class FlatGradBucket:
             for i, n in enumerate(self.names):
                 v = self.views[n]
                 segs[i].g, segs[i].width, segs[i].dense = v.data_ptr(), v.numel() // self.n_gauss, int(n in self.dense_params)
-            stream = ctypes.c_void_p(torch.cuda.current_stream().cuda_stream)
+            stream = L.stream()
             L.check(_timed("bucket_zero", L.load().dnr_grad_zero, ctypes.cast(segs, ctypes.c_void_p), len(segs),
                            self.touched.data_ptr(), self.n_gauss, stream), "dnr_grad_zero")
         else:

@@ -25,7 +25,7 @@ from torch import Tensor
 
 from . import _lib as L
 from .mesh import TriangleMesh, _quantile_sorted, _views, marching_cubes, write_ply
-from .sugar import _need_cuda, _stream, knn_gpu, sample_points_in_gaussians
+from .sugar import knn_gpu, sample_points_in_gaussians
 
 DEFAULT_POINT_WEIGHT = 4.0
 """Screening weight alpha: a node on a uniformly sampled surface is screened with about alpha (in units where the
@@ -70,21 +70,14 @@ def poisson_grid(points: Tensor, depth: int, scale: float = 1.1) -> PoissonGrid:
     return PoissonGrid(tuple(float(c - 0.5 * side) for c in centre), side / (1 << depth), int(depth))
 
 
-def _ws_bytes(fn, *args) -> int:
-    n = int(fn(*args))
-    if n < 0:
-        L.check(n, fn.__name__ if hasattr(fn, "__name__") else "workspace query")
-    return n
-
-
 def required_bytes(depth: int, n_points: int, max_cycles: int = MAX_CYCLES) -> int:
     """Peak device bytes of poisson_reconstruct: the splat workspace with its outputs, then the solver's."""
     lib = L.load()
     g = PoissonGrid((0.0, 0.0, 0.0), 1.0, depth).struct()
     N = (1 << depth) ** 3
     outputs = 4 * N * 4 + 4 * (N // 64) * 4 + 4 * n_points  # S, faces, density, colour grid, weights
-    splat = _ws_bytes(lib.dnr_poisson_splat_workspace_bytes, C.byref(g), max(n_points, 1))
-    solve = _ws_bytes(lib.dnr_poisson_solve_workspace_bytes, C.byref(g), max_cycles) + 4 * N  # + chi
+    splat = L.workspace_bytes(lib.dnr_poisson_splat_workspace_bytes, C.byref(g), max(n_points, 1))
+    solve = L.workspace_bytes(lib.dnr_poisson_solve_workspace_bytes, C.byref(g), max_cycles) + 4 * N  # + chi
     return outputs + max(splat, solve)
 
 
@@ -99,7 +92,7 @@ def _check_budget(depth: int, n: int, max_bytes: int) -> None:
 def _prep(t: Optional[Tensor], n: int, what: str) -> Optional[Tensor]:
     if t is None:
         return None
-    _need_cuda(t)
+    L.need_cuda(t)
     t = t.detach().float().reshape(-1, 3).contiguous()
     if t.shape[0] != n:
         raise ValueError(f"poisson: {what} has {t.shape[0]} rows, points has {n}")
@@ -109,7 +102,7 @@ def _prep(t: Optional[Tensor], n: int, what: str) -> Optional[Tensor]:
 def poisson_splat(points: Tensor, normals: Tensor, colors: Optional[Tensor], grid: PoissonGrid) -> Dict[str, Tensor]:
     """dnr_poisson_splat: {"screen" [R^3], "faces" [3,R^3], "density" [(R/4)^3], "colors" [(R/4)^3,4] ({sum a w c, sum a w}) or None,
     "weights" [n] (a_p, mean 1), "area_scale" [1]} on the device."""
-    _need_cuda(points)
+    L.need_cuda(points)
     p = points.detach().float().reshape(-1, 3).contiguous()
     n = p.shape[0]
     if n == 0:
@@ -117,8 +110,7 @@ def poisson_splat(points: Tensor, normals: Tensor, colors: Optional[Tensor], gri
     nrm, col = _prep(normals, n, "normals"), _prep(colors, n, "colors")
     lib, dev, R = L.load(), p.device, grid.R
     g = grid.struct()
-    nbytes = _ws_bytes(lib.dnr_poisson_splat_workspace_bytes, C.byref(g), n)
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    ws, nbytes = L.workspace(lib.dnr_poisson_splat_workspace_bytes, C.byref(g), n, device=dev)
     f32 = dict(dtype=torch.float32, device=dev)
     out = {"screen": torch.empty(R ** 3, **f32), "faces": torch.empty(3, R ** 3, **f32),
            "density": torch.empty((R // 4) ** 3, **f32), "colors": None if col is None else torch.empty((R // 4) ** 3, 4, **f32),
@@ -126,7 +118,7 @@ def poisson_splat(points: Tensor, normals: Tensor, colors: Optional[Tensor], gri
     ptr = lambda t: None if t is None else t.data_ptr()  # noqa: E731
     L.check(lib.dnr_poisson_splat(C.byref(g), p.data_ptr(), nrm.data_ptr(), ptr(col), n, ws.data_ptr(), nbytes,
                                   out["screen"].data_ptr(), out["faces"].data_ptr(), out["density"].data_ptr(), ptr(out["colors"]),
-                                  out["weights"].data_ptr(), out["area_scale"].data_ptr(), _stream()), "dnr_poisson_splat")
+                                  out["weights"].data_ptr(), out["area_scale"].data_ptr(), L.stream()), "dnr_poisson_splat")
     return out
 
 
@@ -135,20 +127,19 @@ def poisson_solve(grid: PoissonGrid, screen: Tensor, faces: Tensor, screen_weigh
     """dnr_poisson_solve: chi [R^3] and the relative residual before the first and after each V-cycle."""
     lib, dev = L.load(), screen.device
     g = grid.struct()
-    nbytes = _ws_bytes(lib.dnr_poisson_solve_workspace_bytes, C.byref(g), int(max_cycles))
-    ws = torch.empty(nbytes, dtype=torch.uint8, device=dev)
+    ws, nbytes = L.workspace(lib.dnr_poisson_solve_workspace_bytes, C.byref(g), int(max_cycles), device=dev)
     chi = torch.empty(grid.R ** 3, dtype=torch.float32, device=dev)
     hist = (C.c_float * (max_cycles + 1))()
     cycles = C.c_int32(0)
     L.check(lib.dnr_poisson_solve(C.byref(g), screen.data_ptr(), faces.data_ptr(), float(screen_weight), float(tol), int(max_cycles),
-                                  ws.data_ptr(), nbytes, chi.data_ptr(), hist, C.byref(cycles), _stream()), "dnr_poisson_solve")
+                                  ws.data_ptr(), nbytes, chi.data_ptr(), hist, C.byref(cycles), L.stream()), "dnr_poisson_solve")
     return chi, [float(hist[i]) for i in range(cycles.value + 1)]
 
 
 def grid_sample(values: Tensor, origin: Sequence[float], cell: float, points: Tensor) -> Tensor:
     """dnr_grid_sample: trilinear interpolation of a cell-centred grid values [X,Y,Z] or [X,Y,Z,C] (node (i,j,k) at
     origin + (index + 0.5) * cell) at points [n,3], clamped to the outer node centres.  Returns [n] or [n,C]."""
-    _need_cuda(values, points)
+    L.need_cuda(values, points)
     v = values.detach().float().contiguous()
     ch = 1 if v.dim() == 3 else v.shape[3]
     d = L.DnrGridDesc()
@@ -157,7 +148,7 @@ def grid_sample(values: Tensor, origin: Sequence[float], cell: float, points: Te
     d.dims[0], d.dims[1], d.dims[2] = v.shape[:3]
     p = points.detach().float().reshape(-1, 3).contiguous()
     out = torch.empty((p.shape[0], ch), dtype=torch.float32, device=p.device)
-    L.check(L.load().dnr_grid_sample(C.byref(d), v.data_ptr(), p.data_ptr(), p.shape[0], out.data_ptr(), _stream()), "dnr_grid_sample")
+    L.check(L.load().dnr_grid_sample(C.byref(d), v.data_ptr(), p.data_ptr(), p.shape[0], out.data_ptr(), L.stream()), "dnr_grid_sample")
     return out[:, 0] if v.dim() == 3 else out
 
 
@@ -231,7 +222,7 @@ def remove_statistical_outlier(points: Tensor, nb_neighbors: int = 20, std_ratio
     """Open3D's PointCloud.remove_statistical_outlier [EXT]: the mean distance of each point to its nb_neighbors nearest
     points, the point itself included (distance 0), kept where <= mean + std_ratio * std (sample std) over the cloud.
     Returns the kept indices (ascending)."""
-    _need_cuda(points)
+    L.need_cuda(points)
     p = points.detach().float().reshape(-1, 3).contiguous()
     n = p.shape[0]
     if n <= nb_neighbors:

@@ -196,10 +196,6 @@ def _ptr(t: Optional[Tensor]) -> Optional[int]:
     return None if t is None else t.data_ptr()
 
 
-def _stream() -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _require_cuda(*ts: Tensor) -> torch.device:
     dev = ts[0].device
     if dev.type != "cuda":
@@ -287,7 +283,7 @@ class _DnRasterize(torch.autograd.Function):
         lists_x, lists_y = (W + list_tile - 1) // list_tile, (H + list_tile - 1) // list_tile
         n_tiles = lists_x * lists_y
         rec_f = L.REC_FLOATS_N if s.render_normals else L.REC_FLOATS
-        st = _stream()
+        st = L.stream()
         ctx.fwd_stream = torch.cuda.current_stream()
         ctx.capacity_ticket = None
 
@@ -403,7 +399,7 @@ class _DnRasterize(torch.autograd.Function):
         S = ctx.state
         n, dev = ctx.n, means.device
         f32 = dict(dtype=torch.float32, device=dev)
-        st = _stream()
+        st = L.stream()
 
         def prep(g):
             # zero-stride tokens stand for "this gradient is evaluated inside dnr_raster_bwd" (deferred losses, below)

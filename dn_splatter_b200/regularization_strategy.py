@@ -26,10 +26,6 @@ from .losses import DepthLoss, DepthLossType, NormalLoss, NormalLossType
 _FUSED_DEPTH = {DepthLossType.EdgeAwareLogL1: 1, DepthLossType.LogL1: 2, DepthLossType.L1: 3, DepthLossType.MSE: 4}
 
 
-def _stream() -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
 def _shared_holder(*tensors):
     """The dn_rasterize holder shared by all the given rendered maps (None if any map is not a direct raster output or
     they come from different renders): only then can a loss hand its backward to dnr_raster_bwd."""
@@ -87,7 +83,7 @@ class _FusedDNLoss(torch.autograd.Function):
         for k, t in dict(out_depth=pd, out_normal=pn, gt_depth=gd, gt_normal=gn, gt_rgb=gi, gt_image=ei,
                          loss_partials=partials).items():
             setattr(a, k, None if t is None else t.data_ptr())
-        L.check(lib.dnr_loss_fwd(C.byref(a), _stream()), "dnr_loss_fwd")
+        L.check(lib.dnr_loss_fwd(C.byref(a), L.stream()), "dnr_loss_fwd")
         ctx.keep = (pd, pn, gd, gn, gi, ei, partials)
         ctx.fwd_stream = torch.cuda.current_stream()
         ctx.cfg = (W, H, int(depth_type), int(bool(use_normal)), float(depth_lambda), float(depth_tolerance), flags)
@@ -127,7 +123,7 @@ class _FusedDNLoss(torch.autograd.Function):
         vn = torch.empty(ctx.shapes[1], dtype=torch.float32, device=v.device) if (use_normal and ctx.needs_input_grad[1]) else None
         if vd is not None or vn is not None:
             L.check(lib.dnr_loss_bwd(C.byref(a), None if vd is None else vd.data_ptr(),
-                                     None if vn is None else vn.data_ptr(), _stream()), "dnr_loss_bwd")
+                                     None if vn is None else vn.data_ptr(), L.stream()), "dnr_loss_bwd")
         return (vd, vn) + none9
 
 
@@ -141,7 +137,7 @@ class _ScaleLoss(torch.autograd.Function):
             raise L.DnrError("scale loss: CUDA tensor required (no CPU path)")
         s = scales.detach().float().contiguous()
         out = torch.empty(1, dtype=torch.float32, device=s.device)
-        L.check(lib.dnr_scale_loss_fwd(s.data_ptr(), s.shape[0], out.data_ptr(), _stream()), "dnr_scale_loss_fwd")
+        L.check(lib.dnr_scale_loss_fwd(s.data_ptr(), s.shape[0], out.data_ptr(), L.stream()), "dnr_scale_loss_fwd")
         ctx.s = s
         ctx.fwd_stream = torch.cuda.current_stream()
         return out[0].clone()
@@ -157,7 +153,7 @@ class _ScaleLoss(torch.autograd.Function):
         s = ctx.s
         v = v.detach().float().contiguous()
         g = torch.empty_like(s)
-        L.check(lib.dnr_scale_loss_bwd(s.data_ptr(), s.shape[0], v.data_ptr(), g.data_ptr(), _stream()),
+        L.check(lib.dnr_scale_loss_bwd(s.data_ptr(), s.shape[0], v.data_ptr(), g.data_ptr(), L.stream()),
                 "dnr_scale_loss_bwd")
         return g
 
@@ -177,7 +173,7 @@ class FusedL1(torch.autograd.Function):
             g = g.float()
         assert g.numel() == p.numel(), "pred / gt size mismatch"
         out = torch.empty(1, dtype=torch.float32, device=p.device)
-        L.check(lib.dnr_l1_fwd(p.data_ptr(), g.data_ptr(), p.numel(), int(g.dtype == torch.uint8), out.data_ptr(), _stream()),
+        L.check(lib.dnr_l1_fwd(p.data_ptr(), g.data_ptr(), p.numel(), int(g.dtype == torch.uint8), out.data_ptr(), L.stream()),
                 "dnr_l1_fwd")
         ctx.keep = (p, g)
         ctx.shape = pred.shape
@@ -202,7 +198,7 @@ class FusedL1(torch.autograd.Function):
             return zero_token(p.view(ctx.shape)), None, None
         vp = torch.empty_like(p)
         L.check(lib.dnr_l1_bwd(p.data_ptr(), g.data_ptr(), p.numel(), int(g.dtype == torch.uint8), v.data_ptr(), vp.data_ptr(),
-                               _stream()), "dnr_l1_bwd")
+                               L.stream()), "dnr_l1_bwd")
         return vp.view(ctx.shape), None, None
 
 
@@ -226,7 +222,7 @@ class FusedSSIM(torch.autograd.Function):
         dmaps = torch.empty((3, H, W, Cn), dtype=torch.float32, device=p.device)
         out = torch.empty(1, dtype=torch.float32, device=p.device)
         L.check(lib.dnr_ssim_fwd_ex(p.data_ptr(), g.data_ptr(), int(g.dtype == torch.uint8), H, W, Cn, dmaps.data_ptr(),
-                                    out.data_ptr(), _stream()), "dnr_ssim_fwd_ex")
+                                    out.data_ptr(), L.stream()), "dnr_ssim_fwd_ex")
         ctx.keep = (p, g, dmaps)
         ctx.fwd_stream = torch.cuda.current_stream()
         return out[0] / float((H - 10) * (W - 10) * Cn)
@@ -240,7 +236,7 @@ class FusedSSIM(torch.autograd.Function):
             vp = torch.empty_like(p)
             H, W, Cn = p.shape
             L.check(lib.dnr_ssim_bwd_ex(p.data_ptr(), g.data_ptr(), int(g.dtype == torch.uint8), H, W, Cn, dmaps.data_ptr(),
-                                        v.data_ptr(), vp.data_ptr(), _stream()), "dnr_ssim_bwd_ex")
+                                        v.data_ptr(), vp.data_ptr(), L.stream()), "dnr_ssim_bwd_ex")
             return vp, None
 
 
@@ -264,7 +260,7 @@ class FusedPhotometric(torch.autograd.Function):
         dmaps = torch.empty((3, H, W, Cn), dtype=torch.float32, device=p.device)
         out = torch.empty(3, dtype=torch.float32, device=p.device)
         L.check(lib.dnr_photometric_fwd(p.data_ptr(), g.data_ptr(), int(g.dtype == torch.uint8), H, W, Cn, float(ssim_lambda),
-                                        dmaps.data_ptr(), out.data_ptr(), _stream()), "dnr_photometric_fwd")
+                                        dmaps.data_ptr(), out.data_ptr(), L.stream()), "dnr_photometric_fwd")
         ctx.keep = (p, g, dmaps)
         ctx.lam = float(ssim_lambda)
         ctx.fwd_stream = torch.cuda.current_stream()
@@ -279,7 +275,7 @@ class FusedPhotometric(torch.autograd.Function):
             vp = torch.empty_like(p)
             H, W, Cn = p.shape
             L.check(lib.dnr_photometric_bwd(p.data_ptr(), g.data_ptr(), int(g.dtype == torch.uint8), H, W, Cn, ctx.lam,
-                                            dmaps.data_ptr(), v.data_ptr(), vp.data_ptr(), _stream()), "dnr_photometric_bwd")
+                                            dmaps.data_ptr(), v.data_ptr(), vp.data_ptr(), L.stream()), "dnr_photometric_bwd")
             return vp, None, None
 
 
@@ -287,7 +283,7 @@ def u8_to_float(img: Tensor, divisor: float = 255.0, clamp_min: float = 0.0) -> 
     """uint8 CUDA image -> fp32 (/divisor, clamped from below) in one kernel (get_gt_img + clamp of the reference)."""
     src = img.contiguous()
     dst = torch.empty(src.shape, dtype=torch.float32, device=src.device)
-    L.check(L.load().dnr_u8_to_f32(src.data_ptr(), src.numel(), float(divisor), float(clamp_min), dst.data_ptr(), _stream()),
+    L.check(L.load().dnr_u8_to_f32(src.data_ptr(), src.numel(), float(divisor), float(clamp_min), dst.data_ptr(), L.stream()),
             "dnr_u8_to_f32")
     return dst
 

@@ -21,6 +21,10 @@ import torch
 from torch import Tensor
 
 from . import _lib as L
+# module-level names that this module's functions look up at call time: the CPU proxy tests substitute _need_cuda here
+# to run the host logic on CPU tensors, and the GPU kernel tests take the stream from here
+from ._lib import need_cuda as _need_cuda
+from ._lib import stream as _stream
 
 KNN = 16
 MAX_DIM = 256
@@ -47,16 +51,6 @@ def _grid_struct(g: Dict) -> "L.DnrKnnGrid":
     return s
 
 
-def _stream() -> C.c_void_p:
-    return C.c_void_p(torch.cuda.current_stream().cuda_stream)
-
-
-def _need_cuda(*ts: Tensor) -> None:
-    for t in ts:
-        if t.device.type != "cuda":
-            raise L.DnrError("dn_splatter_b200.sugar needs CUDA tensors (no CPU path)")
-
-
 class KnnIndex:
     """Grid-hash index over a point set; `query(y, k, skip_first)` mirrors knn_sk(x, y, k) when skip_first=True."""
 
@@ -69,10 +63,7 @@ class KnnIndex:
         self.grid = choose_grid(stats[0].tolist(), stats[1].tolist(), stats[2].tolist(), stats[3].tolist(), n)
         self._g = _grid_struct(self.grid)
         lib = L.load()
-        nbytes = lib.dnr_knn_workspace_bytes(n, C.byref(self._g))
-        if nbytes < 0:
-            raise L.DnrError("dnr_knn_workspace_bytes: bad grid")
-        self.ws = torch.empty(nbytes, dtype=torch.uint8, device=points.device)
+        self.ws, nbytes = L.workspace(lib.dnr_knn_workspace_bytes, n, C.byref(self._g), device=points.device)
         L.check(lib.dnr_knn_build(self.points.data_ptr(), n, C.byref(self._g), self.ws.data_ptr(), nbytes, _stream()), "dnr_knn_build")
 
     def query(self, queries: Tensor, k: int, skip_first: bool = True, return_distances: bool = False):

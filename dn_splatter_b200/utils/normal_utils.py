@@ -27,8 +27,7 @@ def normal_from_depth_image(depths: Tensor, fx: float, fy: float, cx: float, cy:
     a.flags = L.FLAG_HOST_CAMERA  # intrinsics by value: no upload
     a.host_cam[16], a.host_cam[17], a.host_cam[18], a.host_cam[19] = float(fx), float(fy), float(cx), float(cy)
     a.out_depth, a.out_surface_normal = d.data_ptr(), out.data_ptr()
-    st = C.c_void_p(torch.cuda.current_stream().cuda_stream)
-    L.check(L.load().dnr_normal_from_depth(C.byref(a), st), "dnr_normal_from_depth")
+    L.check(L.load().dnr_normal_from_depth(C.byref(a), L.stream()), "dnr_normal_from_depth")
     if c2w is not None and c2w.device.type == "cpu":  # identity test on the host only (a device tensor would sync)
         R = c2w[..., :3, :3].to(out)
         if not bool(torch.equal(c2w[..., :3, :3].float(), torch.eye(3))):

@@ -24,6 +24,10 @@
  * queries).  All work is enqueued on the stream passed in (a cudaStream_t cast to void*); the only
  * host synchronisation is the documented n_isects read-back inside dnr_bin_scan.
  * Return value: 0 = ok, <0 = DNR_E_* argument error, >0 = cudaError_t of a failed launch.
+ * Workspaces: the cub scratch in a workspace is sized by cub's queries, which need a device; without one they fail and
+ * the size a *_workspace_bytes query returns lacks that scratch.  Every entry point that runs cub repeats the queries and,
+ * after DNR_E_WORKSPACE for a workspace that is too small, returns the first failed query's cudaError_t (> 0) rather
+ * than run without the scratch.
  * No global state, re-entrant, never throws, never prints.
  */
 #ifndef DNR_H_
@@ -550,8 +554,6 @@ int dnr_dn_backproject(const float* depth, int32_t width, int32_t height, const 
  * 2 x u64) += (candidates examined, searches run), one search per distinct position; for tests, cov [n,9] the covariance of
  * each point's neighbours and neighbours [n,k] the smallest point index of each neighbour's position, one entry per copy
  * taken, -1 past min(k, n). */
-/* The cub scratch in the workspace is sized by cub's queries, which need a device; without one they fail and the size
- * returned lacks that scratch.  dnr_dn_normals repeats the queries and returns their cudaError_t (> 0) if they fail. */
 int64_t dnr_dn_normals_workspace_bytes(int64_t n_points);
 int dnr_dn_normals(const double* points, int64_t n_points, const DnrDnSearch* search, void* ws, int64_t ws_bytes, double* normals,
                    int32_t* examined, double* cov, int32_t* neighbours, unsigned long long* stats, void* stream);

@@ -184,6 +184,8 @@ def test_abi_argument_errors(lib):
     assert lib.dnr_iso_samples_workspace_bytes(C.byref(fr), 0) == -2
     cnt = C.c_int64()
     assert lib.dnr_iso_samples(C.byref(fr), 1, None, 0, None, None, C.byref(cnt), None) == -1
+    ws = lib.dnr_iso_samples_workspace_bytes(C.byref(fr), 1)
+    assert lib.dnr_iso_samples(C.byref(fr), 1, 16, ws - 1, 16, None, C.byref(cnt), None) == -5
     p = L.DnrIsoParams()
     assert lib.dnr_iso_eval(C.byref(fr), None, None, 1, None, None) == -1
     assert lib.dnr_iso_eval(C.byref(fr), C.byref(p), None, 1, None, None) == -2  # no pass
@@ -202,7 +204,12 @@ def test_abi_argument_errors(lib):
     g.cell = 0.1
     counts = (C.c_int64 * 11)()
     assert lib.dnr_iso_octree(C.byref(g), None, 10, None, 0, counts, None) == -1
+    ws = lib.dnr_iso_octree_workspace_bytes(C.byref(g), 10)
+    assert lib.dnr_iso_octree(C.byref(g), 16, 10, 16, ws - 1, counts, None) == -5
     assert lib.dnr_iso_corners_workspace_bytes(C.byref(g), 0) == -2
+    counts[0] = 1
+    ws, n_corners = lib.dnr_iso_corners_workspace_bytes(C.byref(g), 1), C.c_int64()
+    assert lib.dnr_iso_corners(C.byref(g), 16, counts, 16, ws - 1, 16, 16, 16, 16, C.byref(n_corners), None) == -5
     assert lib.dnr_iso_fill(C.byref(g), None, counts, None, None, None, None) == -1
 
 
