@@ -22,6 +22,7 @@ from torch import Tensor
 
 from . import _lib as L
 from .losses import DepthLoss, DepthLossType, NormalLoss, NormalLossType
+from .rasterize import _timed
 
 _FUSED_DEPTH = {DepthLossType.EdgeAwareLogL1: 1, DepthLossType.LogL1: 2, DepthLossType.L1: 3, DepthLossType.MSE: 4}
 
@@ -83,7 +84,7 @@ class _FusedDNLoss(torch.autograd.Function):
         for k, t in dict(out_depth=pd, out_normal=pn, gt_depth=gd, gt_normal=gn, gt_rgb=gi, gt_image=ei,
                          loss_partials=partials).items():
             setattr(a, k, None if t is None else t.data_ptr())
-        L.check(lib.dnr_loss_fwd(C.byref(a), L.stream()), "dnr_loss_fwd")
+        L.check(_timed("loss_fwd", lib.dnr_loss_fwd, C.byref(a), L.stream()), "dnr_loss_fwd")
         ctx.keep = (pd, pn, gd, gn, gi, ei, partials)
         ctx.fwd_stream = torch.cuda.current_stream()
         ctx.cfg = (W, H, int(depth_type), int(bool(use_normal)), float(depth_lambda), float(depth_tolerance), flags)
@@ -137,7 +138,8 @@ class _ScaleLoss(torch.autograd.Function):
             raise L.DnrError("scale loss: CUDA tensor required (no CPU path)")
         s = scales.detach().float().contiguous()
         out = torch.empty(1, dtype=torch.float32, device=s.device)
-        L.check(lib.dnr_scale_loss_fwd(s.data_ptr(), s.shape[0], out.data_ptr(), L.stream()), "dnr_scale_loss_fwd")
+        L.check(_timed("scale_loss_fwd", lib.dnr_scale_loss_fwd, s.data_ptr(), s.shape[0], out.data_ptr(), L.stream()),
+                "dnr_scale_loss_fwd")
         ctx.s = s
         ctx.fwd_stream = torch.cuda.current_stream()
         return out[0].clone()
@@ -153,8 +155,8 @@ class _ScaleLoss(torch.autograd.Function):
         s = ctx.s
         v = v.detach().float().contiguous()
         g = torch.empty_like(s)
-        L.check(lib.dnr_scale_loss_bwd(s.data_ptr(), s.shape[0], v.data_ptr(), g.data_ptr(), L.stream()),
-                "dnr_scale_loss_bwd")
+        L.check(_timed("scale_loss_bwd", lib.dnr_scale_loss_bwd, s.data_ptr(), s.shape[0], v.data_ptr(), g.data_ptr(),
+                       L.stream()), "dnr_scale_loss_bwd")
         return g
 
 
@@ -259,8 +261,8 @@ class FusedPhotometric(torch.autograd.Function):
         H, W, Cn = p.shape
         dmaps = torch.empty((3, H, W, Cn), dtype=torch.float32, device=p.device)
         out = torch.empty(3, dtype=torch.float32, device=p.device)
-        L.check(lib.dnr_photometric_fwd(p.data_ptr(), g.data_ptr(), int(g.dtype == torch.uint8), H, W, Cn, float(ssim_lambda),
-                                        dmaps.data_ptr(), out.data_ptr(), L.stream()), "dnr_photometric_fwd")
+        L.check(_timed("photometric_fwd", lib.dnr_photometric_fwd, p.data_ptr(), g.data_ptr(), int(g.dtype == torch.uint8), H, W,
+                       Cn, float(ssim_lambda), dmaps.data_ptr(), out.data_ptr(), L.stream()), "dnr_photometric_fwd")
         ctx.keep = (p, g, dmaps)
         ctx.lam = float(ssim_lambda)
         ctx.fwd_stream = torch.cuda.current_stream()
@@ -274,8 +276,8 @@ class FusedPhotometric(torch.autograd.Function):
             v = v.detach().float().contiguous()
             vp = torch.empty_like(p)
             H, W, Cn = p.shape
-            L.check(lib.dnr_photometric_bwd(p.data_ptr(), g.data_ptr(), int(g.dtype == torch.uint8), H, W, Cn, ctx.lam,
-                                            dmaps.data_ptr(), v.data_ptr(), vp.data_ptr(), L.stream()), "dnr_photometric_bwd")
+            L.check(_timed("photometric_bwd", lib.dnr_photometric_bwd, p.data_ptr(), g.data_ptr(), int(g.dtype == torch.uint8), H,
+                           W, Cn, ctx.lam, dmaps.data_ptr(), v.data_ptr(), vp.data_ptr(), L.stream()), "dnr_photometric_bwd")
             return vp, None, None
 
 

@@ -238,8 +238,9 @@ int dnr_u8_to_f32(const uint8_t* src, int64_t n, float divisor, float clamp_min,
 /* SSIM term of the same photometric loss: torchmetrics StructuralSimilarityIndexMeasure(data_range=1.0,
  * kernel_size=11) (dn_splatter/dn_model.py:180), i.e. an 11x11 Gaussian window (sigma 1.5), mean over the
  * (H-10)x(W-10) interior.  pred / gt: [H,W,C] fp32.  fwd: *sum_out (zeroed by the call) = SUM of the SSIM map over
- * the interior and all channels (divide by (H-10)(W-10)C for the mean); dmaps [3,H,W,C] keeps the partial
- * derivatives for the backward.  bwd: v_pred[H,W,C] = (*v_mean or 1) * d(mean SSIM)/d(pred).
+ * the interior and all channels (divide by (H-10)(W-10)C for the mean); dmaps: 3·H·W·C floats of scratch whose
+ * layout is private to the pair, written by the forward and read by the backward.
+ * bwd: v_pred[H,W,C] = (*v_mean or 1) * d(mean SSIM)/d(pred).
  * Default since round 2 (DNSplatterModelConfig.fused_ssim). */
 int dnr_ssim_fwd(const float* pred, const float* gt, int32_t H, int32_t W, int32_t C, float* dmaps, float* sum_out,
                  void* stream);
