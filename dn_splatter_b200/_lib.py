@@ -47,6 +47,18 @@ class DnrArgs(C.Structure):
     ]
 
 
+class DnrAgsLoss(C.Structure):
+    """Mirror of struct DnrAgsLoss (include/dnr.h)."""
+
+    _fields_ = [("width", _i), ("height", _i), ("depth_loss_type", _i), ("flags", C.c_uint32), ("depth_lambda", _f),
+                ("depth_tolerance", _f), ("normal_lambda", _f), ("reserved", _i), ("pred_depth", _p), ("gt_depth", _p),
+                ("confidence", _p), ("image", _p), ("surf_normal", _p), ("gt_normal", _p), ("pred_normal", _p),
+                ("partials", _p), ("v_loss", _p), ("keep_mask", _p)]
+
+
+AGS_CONF_GATE, AGS_ANGLE_MASK, AGS_NORMAL_U8, AGS_IMG_U8, AGS_CONF_RAW, AGS_CONF_U8, AGS_SIGNED_CHW = 1, 2, 4, 8, 16, 32, 64
+
+
 class DnrAdamSeg(C.Structure):
     """Mirror of struct DnrAdamSeg (include/dnr.h)."""
 
@@ -148,7 +160,7 @@ _lib: Optional[C.CDLL] = None
 KERNELS_PER_CALL = {
     "dnr_project_fwd": (1, 0), "dnr_bin_scan": (2, 8), "dnr_bin_sort": (3, 4), "dnr_raster_fwd": (1, 0),
     "dnr_finalize_fwd": (1, 0), "dnr_normal_from_depth": (1, 0), "dnr_raster_bwd": (1, 0), "dnr_project_bwd": (1, 0),
-    "dnr_loss_fwd": (2, 0), "dnr_loss_bwd": (1, 0), "dnr_scale_loss_fwd": (1, 0), "dnr_scale_loss_bwd": (1, 0),
+    "dnr_loss_fwd": (2, 0), "dnr_loss_bwd": (1, 0), "dnr_ags_loss_fwd": (2, 0), "dnr_ags_loss_bwd": (1, 0), "dnr_scale_loss_fwd": (1, 0), "dnr_scale_loss_bwd": (1, 0),
     "dnr_l1_fwd": (1, 0), "dnr_l1_bwd": (1, 0), "dnr_u8_to_f32": (1, 0),
     "dnr_ssim_fwd": (1, 0), "dnr_ssim_bwd": (1, 0), "dnr_ssim_fwd_ex": (1, 0), "dnr_ssim_bwd_ex": (1, 0), "dnr_photometric_fwd": (2, 0), "dnr_photometric_bwd": (1, 0), "dnr_adam_step": (1, 0), "dnr_adam_step_reduce": (2, 0),
     "dnr_grad_zero": (1, 0),
@@ -227,6 +239,10 @@ def load():
     lib.dnr_bin_scan.argtypes = [A, C.c_void_p, C.POINTER(C.c_int64)]
     lib.dnr_loss_bwd.restype = C.c_int
     lib.dnr_loss_bwd.argtypes = [A, C.c_void_p, C.c_void_p, C.c_void_p]
+    lib.dnr_ags_loss_fwd.restype = C.c_int
+    lib.dnr_ags_loss_fwd.argtypes = [C.POINTER(DnrAgsLoss), C.c_void_p]
+    lib.dnr_ags_loss_bwd.restype = C.c_int
+    lib.dnr_ags_loss_bwd.argtypes = [C.POINTER(DnrAgsLoss), C.c_void_p, C.c_void_p, C.c_void_p]
     lib.dnr_scale_loss_fwd.restype = C.c_int
     lib.dnr_scale_loss_fwd.argtypes = [C.c_void_p, C.c_int32, C.c_void_p, C.c_void_p]
     lib.dnr_scale_loss_bwd.restype = C.c_int
@@ -353,7 +369,7 @@ def load():
 EXPORTS = (
     "dnr_version", "dnr_error_string", "dnr_project_fwd", "dnr_bin_scan_workspace_bytes", "dnr_bin_scan",
     "dnr_bin_sort_workspace_bytes", "dnr_bin_sort", "dnr_raster_fwd", "dnr_finalize_fwd", "dnr_normal_from_depth",
-    "dnr_raster_bwd", "dnr_project_bwd", "dnr_loss_fwd", "dnr_loss_bwd", "dnr_scale_loss_fwd", "dnr_scale_loss_bwd",
+    "dnr_raster_bwd", "dnr_project_bwd", "dnr_loss_fwd", "dnr_loss_bwd", "dnr_ags_loss_fwd", "dnr_ags_loss_bwd", "dnr_scale_loss_fwd", "dnr_scale_loss_bwd",
     "dnr_l1_fwd", "dnr_l1_bwd", "dnr_u8_to_f32", "dnr_ssim_fwd", "dnr_ssim_bwd", "dnr_ssim_fwd_ex", "dnr_ssim_bwd_ex", "dnr_photometric_fwd", "dnr_photometric_bwd", "dnr_adam_step", "dnr_adam_step_reduce", "dnr_grad_zero", "dnr_knn_workspace_bytes", "dnr_knn_build", "dnr_knn_query",
     "dnr_density", "dnr_ray_densities", "dnr_tsdf_integrate", "dnr_mc_count_workspace_bytes", "dnr_mc_count",
     "dnr_mc_emit_workspace_bytes", "dnr_mc_emit", "dnr_poisson_splat_workspace_bytes", "dnr_poisson_splat",

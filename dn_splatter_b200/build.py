@@ -20,6 +20,7 @@ COMMON = ["-O3", "-lineinfo", "-std=c++17", "-Xcompiler", "-fPIC", "--expt-relax
 SOURCES = {
     "project.cu": ["-fmad=false"],
     "image_ops.cu": ["-fmad=false"],
+    "ags_loss.cu": ["-fmad=false"],  # 2x - 1, products and sums round as torch's element-wise kernels do
     "binning.cu": [],
     "raster.cu": [],
     "misc.cu": [],

@@ -552,6 +552,32 @@ class DNSplatterModel(_ModelBase):
             z = self.__dict__["_zero_scalar"] = torch.zeros((), device=self.device)
         return z
 
+    def _ags_raw_ok(self, outputs, batch) -> bool:
+        """Whether get_loss_dict hands the batch's maps to AGSMeshRegularization's fused kernels as stored: the ags-mesh
+        strategy on a fused configuration, CUDA maps of a kernel dtype, no batch mask, no downscale, and every map the
+        strategy reads present (a missing one keeps the torch code and its error)."""
+        cfg = self.config
+        rs = self.regularization_strategy
+        if not (cfg.regularization_strategy == "ags-mesh" and rs._fusable() and "mask" not in batch
+                and self._get_downscale_factor() == 1):
+            return False
+        u8f32 = (torch.uint8, torch.float32)
+        image, conf = batch["image"], batch.get("confidence")
+        if not (image.is_cuda and image.shape[-1] == 3 and image.dtype in u8f32):
+            return False
+        if conf is None or not conf.is_cuda or conf.dtype not in u8f32:
+            return False
+        if "sensor_depth" not in batch and "mono_depth" not in batch:
+            return False
+        if cfg.normal_supervision == "mono":
+            n = batch.get("normal")
+            if n is None or not n.is_cuda or n.dtype not in u8f32:
+                return False
+        elif cfg.normal_supervision != "depth":
+            return False
+        maps = (outputs["depth"], outputs["normal"], outputs["surface_normal"])
+        return all(t.is_cuda and t.dtype == torch.float32 for t in maps) and not outputs["surface_normal"].requires_grad
+
     def get_loss_dict(self, outputs, batch, metrics_dict=None) -> Dict[str, Tensor]:
         cfg = self.config
         loss_dict = self._rgb_loss_dict(outputs, batch)
@@ -560,13 +586,18 @@ class DNSplatterModel(_ModelBase):
         # uint8 maps go to the fused regulariser as they are (scaled and clamped inside the kernels): no conversion passes
         raw_ok = (cfg.regularization_strategy == "dn-splatter" and "mask" not in batch and self._get_downscale_factor() == 1
                   and image.dtype == torch.uint8 and image.is_cuda and image.shape[-1] == 3)
-        gt_img = image if raw_ok else self.get_gt_img(image, clamp_min=10 / 255.0)  # quirk B10
+        # ags-mesh on the fused kernels: the raw image, normals and confidence map go to them as stored, the rendered
+        # normals in their [0,1] encoding (no 2x - 1, permute or get_gt_img passes)
+        ags_raw = self._ags_raw_ok(outputs, batch)
+        gt_img = image if (raw_ok or (ags_raw and image.dtype == torch.uint8)) else self.get_gt_img(image, clamp_min=10 / 255.0)  # quirk B10
         depth_out = outputs["depth"]
         sensor_depth_gt = self.get_gt_img(batch["sensor_depth"]) if "sensor_depth" in batch else None
         mono_depth_gt = self.get_gt_img(batch["mono_depth"]) if "mono_depth" in batch else None
-        if "normal" in batch and not (raw_ok and batch["normal"].dtype == torch.uint8 and batch["normal"].is_cuda):
+        if "normal" in batch and not ((raw_ok or ags_raw) and batch["normal"].dtype == torch.uint8 and batch["normal"].is_cuda):
             batch["normal"] = self.get_gt_img(batch["normal"])
-        if "confidence" in batch:
+        if ags_raw:
+            confidence = batch["confidence"]
+        elif "confidence" in batch:
             confidence = 1 - self.get_gt_img(batch["confidence"]) / 255.0
         if "mask" in batch:  # quirk B11: in-place on the dicts
             mask = batch["mask"].to(self.device)
@@ -600,7 +631,11 @@ class DNSplatterModel(_ModelBase):
         if depth_gt is None and cfg.use_depth_loss:
             print("[dn_splatter_b200] use_depth_loss is True but the batch holds no depth maps")
         extra = {"scales": self.scales, "gt_img": gt_img}
-        if cfg.regularization_strategy == "dn-splatter":
+        if ags_raw:
+            reg = self.regularization_strategy.fused_loss(
+                self.step, depth_out, depth_gt, surface_normal, gt_normal, pred_normal, confidence, gt_img, self.scales,
+                confidence_raw=True)
+        elif cfg.regularization_strategy == "dn-splatter":
             reg = self.regularization_strategy(pred_depth=depth_out, gt_depth=depth_gt, pred_normal=pred_normal,
                                                gt_normal=gt_normal, **extra)
         else:

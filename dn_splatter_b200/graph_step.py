@@ -133,8 +133,11 @@ class GraphedTrainStep:
     def _gates(m):
         """Host-side, step-dependent branches of get_outputs / get_loss_dict that a capture bakes in."""
         c = m.config
-        return (min(m.step // c.sh_degree_interval, c.sh_degree), bool(c.use_scale_regularization and m.step % 10 == 0),
-                bool(c.use_binary_opacities and m.step > c.warmup_length), m._get_downscale_factor())
+        gates = (min(m.step // c.sh_degree_interval, c.sh_degree), bool(c.use_scale_regularization and m.step % 10 == 0),
+                 bool(c.use_binary_opacities and m.step > c.warmup_length), m._get_downscale_factor())
+        if c.regularization_strategy == "ags-mesh":  # AGSMeshRegularization's confidence gate, normal weight, mask kind
+            gates += (m.step >= 7000, m.step > 7000, m.step < m.regularization_strategy.normal_mask_steps)
+        return gates
 
     def _capture(self) -> None:
         model = self.model

@@ -6,8 +6,9 @@ DNRegularization is the hot path: its depth term (EdgeAwareLogL1 / LogL1 / L1 / 
 normal L1 + TV and min-scale term are evaluated by fused CUDA kernels (dnr_loss_fwd / dnr_loss_bwd /
 dnr_scale_loss_*: one pass over the rendered maps each way instead of ~40 torch kernels and two boolean-mask
 gathers with host syncs).  Loss types the kernels do not cover (Pearson, Huber, ...) run through the torch
-modules of losses.py.  AGSMeshRegularization is API-compatible and executed with torch ops (step-gated,
-mask-indexed; SURVEY.md §2.1 #2).  The reference's quirks are reproduced, not fixed (SURVEY Appendix B6-B9).
+modules of losses.py.  AGSMeshRegularization's depth and normal terms run in the same way on dnr_ags_loss_fwd /
+dnr_ags_loss_bwd, with the step gates passed as flags; its configurations the kernels do not cover keep the torch ops
+(step-gated, mask-indexed; SURVEY.md §2.1 #2).  The reference's quirks are reproduced, not fixed (SURVEY Appendix B6-B9).
 """
 from __future__ import annotations
 
@@ -126,6 +127,78 @@ class _FusedDNLoss(torch.autograd.Function):
             L.check(lib.dnr_loss_bwd(C.byref(a), None if vd is None else vd.data_ptr(),
                                      None if vn is None else vn.data_ptr(), L.stream()), "dnr_loss_bwd")
         return (vd, vn) + none9
+
+
+class _FusedAGSLoss(torch.autograd.Function):
+    """AGSMeshRegularization's depth + normal terms in one kernel each way (include/dnr.h dnr_ags_loss_*); differentiable
+    w.r.t. `pred_depth` and `pred_normal`.  The surface normal is value-only (it comes from detached depth).
+
+    `cfg` = (depth_type, depth_lambda, depth_tolerance, normal_lambda, flags): the step gates arrive already decided as
+    flags (DNR_AGS_CONF_GATE, DNR_AGS_ANGLE_MASK) and as normal_lambda (0 while step <= 7000).  The normal maps are
+    [H,W,3] in the [0,1] encoding (gt may be uint8) or, with AGS_SIGNED_CHW, fp32 [3,H,W] already signed.  `keep_mask`
+    (uint8 [H,W]) receives the surface term's selection when given."""
+
+    @staticmethod
+    def forward(ctx, pred_depth, pred_normal, gt_depth, confidence, image, surf_normal, gt_normal, cfg, keep_mask=None):
+        lib = L.load()
+        depth_type, depth_lambda, tol, lam, flags = cfg
+        if pred_normal.device.type != "cuda":
+            raise L.DnrError("AGSMeshRegularization: the fused regulariser needs CUDA tensors (no CPU path)")
+        dev = pred_normal.device
+        chw = bool(flags & L.AGS_SIGNED_CHW)
+        H, W = (pred_normal.shape[1], pred_normal.shape[2]) if chw else (pred_normal.shape[0], pred_normal.shape[1])
+
+        def prep(t, n, keep_u8=False):
+            if t is None:
+                return None
+            assert t.numel() == n, f"map of {t.numel()} values where {n} are expected"
+            if keep_u8 and t.dtype == torch.uint8:
+                return t.detach().to(device=dev).contiguous()
+            return t.detach().to(device=dev, dtype=torch.float32).contiguous()
+
+        pn, sn = prep(pred_normal, 3 * H * W), prep(surf_normal, 3 * H * W)
+        gn = prep(gt_normal, 3 * H * W, keep_u8=not chw)
+        pd = prep(pred_depth, H * W) if depth_type else None
+        gd = prep(gt_depth, H * W) if depth_type else None
+        conf = prep(confidence, H * W, keep_u8=bool(flags & L.AGS_CONF_RAW)) if depth_type else None
+        im = prep(image, 3 * H * W, keep_u8=True) if depth_type == 1 else None
+        if gn.dtype == torch.uint8:
+            flags |= L.AGS_NORMAL_U8
+        if im is not None and im.dtype == torch.uint8:
+            flags |= L.AGS_IMG_U8
+        if conf is not None and conf.dtype == torch.uint8:
+            flags |= L.AGS_CONF_U8
+        if not (flags & L.AGS_CONF_GATE):
+            conf = None
+        partials = torch.empty(16, dtype=torch.float32, device=dev)
+        a = L.DnrAgsLoss()
+        a.width, a.height, a.depth_loss_type, a.flags = W, H, int(depth_type), int(flags)
+        a.depth_lambda, a.depth_tolerance, a.normal_lambda = float(depth_lambda), float(tol), float(lam)
+        for k, t in dict(pred_depth=pd, gt_depth=gd, confidence=conf, image=im, surf_normal=sn, gt_normal=gn,
+                         pred_normal=pn, partials=partials, keep_mask=keep_mask).items():
+            setattr(a, k, None if t is None else t.data_ptr())
+        L.check(_timed("ags_loss_fwd", lib.dnr_ags_loss_fwd, C.byref(a), L.stream()), "dnr_ags_loss_fwd")
+        ctx.keep = (pd, gd, conf, im, sn, gn, pn, partials)
+        ctx.args = a
+        ctx.fwd_stream = torch.cuda.current_stream()
+        ctx.shapes = (None if pred_depth is None else pred_depth.shape, pred_normal.shape)
+        return partials[11].clone()
+
+    @staticmethod
+    def backward(ctx, v):
+        with torch.cuda.stream(ctx.fwd_stream):
+            lib = L.load()
+            a = ctx.args
+            v = v.detach().to(torch.float32).contiguous()
+            a.v_loss = v.data_ptr()
+            a.keep_mask = None
+            dev = v.device
+            vd = torch.empty(ctx.shapes[0], dtype=torch.float32, device=dev) if (a.depth_loss_type and ctx.needs_input_grad[0]) else None
+            vn = torch.empty(ctx.shapes[1], dtype=torch.float32, device=dev) if ctx.needs_input_grad[1] else None
+            if vd is not None or vn is not None:
+                L.check(_timed("ags_loss_bwd", lib.dnr_ags_loss_bwd, C.byref(a), None if vd is None else vd.data_ptr(),
+                               None if vn is None else vn.data_ptr(), L.stream()), "dnr_ags_loss_bwd")
+            return (vd, vn) + (None,) * 7
 
 
 class _ScaleLoss(torch.autograd.Function):
@@ -406,7 +479,14 @@ def find_edges(im: Tensor, threshold: float = 0.01, dilation_itr: int = 1) -> Te
 
 
 class AGSMeshRegularization(RegularizationStrategy):
-    """AGS-Mesh filtering strategy (reference :202-327); torch execution, step-gated."""
+    """AGS-Mesh filtering strategy (reference :202-327), step-gated.
+
+    With `fused` (the default) and CUDA maps, a fused depth type (EdgeAwareLogL1 / LogL1 / L1 / MSE) and both losses
+    configured, the depth and normal terms run in one kernel each way (_FusedAGSLoss) and the scale term in the min-scale
+    kernels: no boolean-mask gathers, no host syncs, so a training step that uses it can be captured in a CUDA graph.
+    Everything else runs the torch code below, which restates the reference line by line."""
+
+    fused = True
 
     def __init__(self, depth_tolerance: float = 0.1,
                  depth_loss_type: Optional[DepthLossType] = DepthLossType.EdgeAwareLogL1, depth_lambda: float = 0.2,
@@ -423,7 +503,46 @@ class AGSMeshRegularization(RegularizationStrategy):
         self.normal_mask_steps, self.depth_mask_steps = normal_mask_steps, depth_mask_steps
         self.step = 0
 
+    def _fusable(self) -> bool:
+        return self.fused and self.depth_loss_type in _FUSED_DEPTH and self.depth_loss is not None and self.normal_loss is not None
+
+    def _gates(self, step: int):
+        """(flags, normal lambda) of the step: the confidence gate from 7000 on (hard-coded upstream, not depth_mask_steps),
+        the normal terms from 7001 on, the angular mask instead of the edge mask from normal_mask_steps on."""
+        flags = (L.AGS_CONF_GATE if step >= 7000 else 0) | (0 if step < self.normal_mask_steps else L.AGS_ANGLE_MASK)
+        return flags, (self.normal_lambda if step > 7000 else 0.0)
+
+    def _fused_ok(self, step, pred_depth, gt_depth, surf_normal, gt_normal, pred_normal, confidence_map, gt_img) -> bool:
+        maps = (pred_depth, gt_depth, surf_normal, gt_normal, pred_normal)
+        if not self._fusable() or any(t is None or not t.is_cuda or t.dtype != torch.float32 for t in maps):
+            return False
+        if surf_normal.requires_grad or gt_normal.dim() != 3 or gt_normal.shape[0] != 3:
+            return False
+        if step >= 7000 and (confidence_map is None or not confidence_map.is_cuda or confidence_map.dtype != torch.float32):
+            return False
+        if self.depth_loss_type == DepthLossType.EdgeAwareLogL1:
+            return gt_img is not None and gt_img.is_cuda and gt_img.dtype == torch.float32 and gt_img.shape[-1] == 3
+        return True
+
+    def fused_loss(self, step, pred_depth, gt_depth, surf_normal, gt_normal, pred_normal, confidence, image, scales,
+                   confidence_raw: bool = False, signed_chw: bool = False, keep_mask=None):
+        """get_loss on the fused kernels.  Default layout: `surf_normal`, `gt_normal`, `pred_normal` are [H,W,3] in the
+        [0,1] encoding the model holds (gt fp32 or uint8), `image` the uint8 image (clamped at 10/255 by the kernel) or
+        the fp32 edge image; `confidence_raw`: `confidence` is the batch's map (uint8 or fp32), gated on
+        1 - get_gt_img(c) / 255 > 0.  `signed_chw`: the normals are the signed [3,H,W] maps get_loss receives."""
+        flags, lam = self._gates(step)
+        if confidence_raw:
+            flags |= L.AGS_CONF_RAW
+        if signed_chw:
+            flags |= L.AGS_SIGNED_CHW
+        cfg = (_FUSED_DEPTH[self.depth_loss_type], self.depth_lambda, self.depth_tolerance, lam, flags)
+        reg = _FusedAGSLoss.apply(pred_depth, pred_normal, gt_depth, confidence, image, surf_normal, gt_normal, cfg, keep_mask)
+        return reg + _ScaleLoss.apply(scales)
+
     def get_loss(self, step, pred_depth, gt_depth, surf_normal, gt_normal, pred_normal, confidence_map, **kwargs):
+        if self._fused_ok(step, pred_depth, gt_depth, surf_normal, gt_normal, pred_normal, confidence_map, kwargs.get("gt_img")):
+            return self.fused_loss(step, pred_depth, gt_depth, surf_normal, gt_normal, pred_normal, confidence_map,
+                                   kwargs.get("gt_img"), kwargs["scales"], signed_chw=True)
         d = self.get_depth_loss(step=step, pred_depth=pred_depth, gt_depth=gt_depth, confidence_map=confidence_map, **kwargs)
         n = self.get_normal_loss(step, surf_normal, gt_normal, pred_normal)
         return d + n + self.get_scale_loss(scales=kwargs["scales"])

@@ -221,6 +221,52 @@ int dnr_project_bwd(const DnrArgs* a, void* stream);
 int dnr_loss_fwd(const DnrArgs* a, void* stream);
 int dnr_loss_bwd(const DnrArgs* a, float* v_depth_out, float* v_normal_out, void* stream);
 
+/* AGSMeshRegularization depth + normal terms (dn_splatter/regularization_strategy.py:202-321) on rendered maps.
+ * The step-dependent choices are host flags: DNR_AGS_CONF_GATE (step >= 7000), DNR_AGS_ANGLE_MASK (step >=
+ * normal_mask_steps; else the dilated-edge mask of the gt normal) and normal_lambda, which the caller passes as 0 while
+ * step <= 7000.  Normal maps are [H,W,3] in the [0,1] encoding (the kernels form 2x - 1 in fp32; gt_normal may be uint8,
+ * read as value / 255 with DNR_AGS_NORMAL_U8), or, with DNR_AGS_SIGNED_CHW, fp32 [3,H,W] already signed.
+ * partials (16 floats; [0..11] zeroed by the forward):
+ * [0] sum_x  [1] count_x  [2] sum_y  [3] count_y  (depth term; for non edge-aware types only x is used)
+ * [4] sum |n - g| over all elements  [5] sum |s - g| over the kept elements  [6] their count
+ * [8] depth_lambda * depth term  [9] normal_lambda * surface term  [10] normal_lambda * predicted-normal term
+ * [11] [8] + ([9] + [10]).  An empty depth mask or surface selection makes its term nan, as torch's mean of nothing.
+ * keep_mask (optional, [H,W] uint8): bit c set where element (c, pixel) is in the surface-term selection.
+ * dnr_ags_loss_bwd writes d(loss)/d(pred_depth) [H,W] and d(loss)/d(pred_normal) ([H,W,3], or [3,H,W] with
+ * DNR_AGS_SIGNED_CHW); either may be NULL.  The surface normal gets no gradient (it comes from detached depth). */
+typedef struct DnrAgsLoss {
+  int32_t width, height;
+  int32_t depth_loss_type;  /* 0 none, 1 EdgeAwareLogL1, 2 LogL1, 3 L1, 4 MSE */
+  uint32_t flags;           /* DNR_AGS_* */
+  float depth_lambda, depth_tolerance;
+  float normal_lambda;      /* already gated by the step */
+  int32_t reserved;
+  const float* pred_depth;  /* [H,W] */
+  const float* gt_depth;    /* [H,W] */
+  const void* confidence;   /* [H,W]: the gate map (fp32), or the raw map (DNR_AGS_CONF_RAW: fp32, or uint8 with
+                               DNR_AGS_CONF_U8) gated on conf = 1 - get_gt_img(c) / 255 */
+  const void* image;        /* [H,W,3] edge image of EdgeAwareLogL1: fp32 as given, or uint8 (DNR_AGS_IMG_U8) scaled
+                               by 1/255 and clamped below at 10/255 */
+  const float* surf_normal; /* surface normal of the rendered depth */
+  const void* gt_normal;
+  const float* pred_normal;
+  float* partials;
+  const float* v_loss;      /* upstream gradient of [11] (NULL: 1) */
+  uint8_t* keep_mask;
+} DnrAgsLoss;
+
+#define DNR_AGS_CONF_GATE 1u
+#define DNR_AGS_ANGLE_MASK 2u
+#define DNR_AGS_NORMAL_U8 4u
+#define DNR_AGS_IMG_U8 8u
+#define DNR_AGS_CONF_RAW 16u
+#define DNR_AGS_CONF_U8 32u
+#define DNR_AGS_SIGNED_CHW 64u
+#define DNR_AGS_ALL_FLAGS 127u
+
+int dnr_ags_loss_fwd(const DnrAgsLoss* a, void* stream);
+int dnr_ags_loss_bwd(const DnrAgsLoss* a, float* v_depth_out, float* v_normal_out, void* stream);
+
 /* DNRegularization.get_scale_loss (regularization_strategy.py:195-199): mean_i min_k exp(scales[i,k]).
  * fwd: *loss_out (zeroed by the call) = the mean.  bwd: v_scales[N,3] = v * d(loss)/d(scales) (dense). */
 int dnr_scale_loss_fwd(const float* scales, int32_t n_gauss, float* loss_out, void* stream);
